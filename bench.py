@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- RS encode GB/s at (n,k)=(2^20,2^19), 4 KiB blocks (BASELINE.json metric), on N B200s.
+"""bench.py -- RS encode GB/s at (n,k)=(2^20,2^19), 4 KiB blocks (BASELINE.json metric), on N H100s.
 
 Own arm (default): one process per GPU (torchrun for N>1).  A step = one full encode (RS.cpp:41-63) of N=2^19 data
 blocks x 4096 B -> 2^19 parity blocks.  Throughput convention is the reference's: bytes = 2*N*SIZE*4 per encode (RS.cpp:38).
@@ -15,13 +15,17 @@ must equal the single-GPU encode bit for bit.  A mismatch aborts the run: no lin
 `--impl reference`: times the UNMODIFIED reference CPU encoder (oracle/_ref, compiled from /root/reference by
 oracle/Makefile: AVX2 + OpenMP build, all host threads) on the same config; rank 0 only.
 
+`--dump-outputs DIR`: after the timed steps, rank 0 writes what its last timed step left in the encoded array (the parity
+blocks a caller receives): a fixed, seeded sample of DUMP_ROWS rows as DIR/parity_rows.npy (float64, exact for values < P)
+and their row numbers as DIR/parity_row_index.npy.  The inputs depend only on the arguments, so two builds can be
+compared output for output.
+
 One JSON line on stdout (rank 0).  See DESIGN.md section 7 for how every field is measured.
 """
 import argparse
 import ctypes
 import json
 import os
-import re
 import subprocess
 import sys
 import threading
@@ -68,30 +72,6 @@ def bind_to_gpu_numa_node(local_rank):
         return "not bound (%s)" % type(e).__name__
 
 
-def profiled_traffic():
-    """DRAM bytes (read + write) per ntt_pass_kernel launch from the committed `ncu --set full` capture of this workload
-    (profiles/*_passes_A_BC_D.csv, highest round / version in the name), averaged over the three passes of an encode; None if absent."""
-    import csv
-    import glob
-    import re
-
-    def version(path):                      # r<round>_ncu_v<kernel version>_passes_A_BC_D.csv: newest round, then newest version
-        m = re.search(r"r(\d+)_ncu_v(\d+)_passes", os.path.basename(path))
-        return (int(m.group(1)), int(m.group(2))) if m else (-1, -1)
-    files = sorted(glob.glob(os.path.join(ROOT, "profiles", "r*_ncu_v*_passes_A_BC_D.csv")), key=version)
-    if not files:
-        return None, None
-    try:
-        rows = list(csv.reader(open(files[-1])))
-        h, units, data = rows[0], rows[1], rows[2:]
-        ir, iw = h.index("dram__bytes_read.sum"), h.index("dram__bytes_write.sum")
-        scale = {"Gbyte": 1e9, "Mbyte": 1e6, "Kbyte": 1e3, "byte": 1.0}
-        tot = [float(r[ir]) * scale[units[ir]] + float(r[iw]) * scale[units[iw]] for r in data]
-        return sum(tot) / len(tot), os.path.basename(files[-1])
-    except Exception:
-        return None, None
-
-
 def parse_args():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -107,6 +87,7 @@ def parse_args():
                     help="multi-GPU headline: ONE transform sharded over the GPUs with the exchange fused into the kernels' stores (default; strong scaling, "
                          "BASELINE config 4), the same with two NCCL all-to-alls, or only independent stripes (weak scaling)")
     ap.add_argument("--no-stripes", action="store_true", help="skip the secondary independent-stripes measurement of a multi-GPU run")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write a seeded sample of the last timed step's parity blocks to DIR/*.npy")
     return ap.parse_args()
 
 
@@ -117,11 +98,11 @@ def measured_peak():
             return float(json.load(open(path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet HBM3 bandwidth (not measured)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons sampled during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks/throttle reasons sampled during the timed region (read-only queries)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -251,11 +232,8 @@ def run_reference_arm(args):
     for _ in range(max(1, min(args.warmup, 3))):
         fn()
     times = []
-    budget_t0 = time.perf_counter()
     for _ in range(args.steps):
         t0 = time.perf_counter(); fn(); times.append(time.perf_counter() - t0)
-        if time.perf_counter() - budget_t0 > 240:          # keep the whole run within a few minutes
-            break
     total = sum(times)
     nbytes = 2.0 * N * size_words * 4
     value = nbytes * len(times) / total / 1e9
@@ -291,7 +269,7 @@ def quick_cpu_baseline(args):
         return {"value": None, "unit": "GB/s", "cores": 0, "kind": "unavailable", "sample": repr(e)}
 
 
-# ---------------------------------------------------------------------------------------------------- B200 arm
+# ----------------------------------------------------------------------------------------------------- GPU arm
 def fill_a_rows(torch, dev, first_row, row_step, rows, S):
     """Rows first_row + l*row_step (l < rows) of the reference's fill data0[i] = i % P (RS.cpp:28-29) as an int32 CUDA tensor."""
     out = torch.empty((rows, S), dtype=torch.int32, device=dev)
@@ -302,6 +280,35 @@ def fill_a_rows(torch, dev, first_row, row_step, rows, S):
         r = (torch.arange(lo, hi, device=dev, dtype=torch.int64) * row_step + first_row) * S
         out[lo:hi] = ((r[:, None] + cols[None, :]) % P).to(torch.int32)
     return out
+
+
+DUMP_ROWS = 4096                 # rows of the --dump-outputs sample: 32 MiB of float64 at the headline 4 KiB blocks
+DUMP_BYTES = 64 * 10**6
+
+
+def dump_outputs(out_dir, t):
+    """--dump-outputs: a fixed, seeded sample of the rows of the encoded device array t as float64 (exact: values < P < 2^53)."""
+    import numpy as np
+    import torch
+    rows, S = t.shape
+    n = max(1, min(rows, DUMP_ROWS, DUMP_BYTES // (8 * (S + 1))))
+    idx = np.sort(np.random.default_rng(0).choice(rows, size=n, replace=False))
+    sample = t[torch.from_numpy(idx).to(t.device)].cpu().numpy().view(np.uint32).astype(np.float64)
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "parity_rows.npy"), sample)
+    np.save(os.path.join(out_dir, "parity_row_index.npy"), idx.astype(np.float64))
+
+
+def gpu_identity(index):
+    """Card name and power limit (read-only nvidia-smi query): the timings of a line are only meaningful with them."""
+    try:
+        out = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=name,power.limit", "--format=csv,noheader,nounits"],
+                             capture_output=True, text=True, timeout=60).stdout.strip()
+        name, limit = [x.strip() for x in out.split(",")[:2]]
+        return {"name": name, "power_limit_w": float(limit)}
+    except Exception:                                   # noqa: BLE001 -- the name alone still comes from the runtime
+        import torch
+        return {"name": torch.cuda.get_device_name(index), "power_limit_w": None}
 
 
 def parity_hash(fe, t):
@@ -350,7 +357,7 @@ def run_b200_arm(args):
         os.environ.setdefault("NCCL_DEBUG_FILE", "/dev/stderr")      # keep NCCL's banner off stdout: rank 0 prints exactly one JSON line there
         dist.init_process_group("nccl", device_id=torch.device("cuda", local))
     import fastecc_b200 as fe
-    fe.init(local)                      # raises if the CUDA library or an sm_100 GPU is missing: no fallback
+    fe.init(local)                      # raises if the CUDA library or an sm_90 GPU is missing: no fallback
 
     N, S = 1 << args.log_n, args.block_bytes // 4
     dev = torch.device("cuda", local)
@@ -414,6 +421,8 @@ def run_single_or_stripes(args, fe, rank, world, local, dev, numa):
         time.sleep(0.25)
     ms, launches = time_stripes(args, fe, dev, world, data)
     clocks = sampler.stop() if sampler else None
+    if rank == 0 and args.dump_outputs:
+        dump_outputs(args.dump_outputs, data)
 
     peak, peak_src = measured_peak()
     kernels = per_kernel_roofline(fe, data, nbytes, peak, max(3, min(args.steps, 10))) if rank == 0 else None
@@ -449,7 +458,6 @@ def run_single_or_stripes(args, fe, rank, world, local, dev, numa):
         fe.lib().fastecc_b200_host_free(hptr)
 
     if rank == 0:
-        traffic, traffic_src = profiled_traffic() if (args.log_n == 19 and args.block_bytes == 4096) else (None, None)
         top = max(kernels, key=lambda k: k["ms"]) if kernels else {"kernel": "small_dft_kernel", "pass": "single", "achieved": nbytes / (ms / args.steps * 1e-3) / 1e9,
                                                                    "frac": nbytes / (ms / args.steps * 1e-3) / 1e9 / peak}
         out = {
@@ -461,11 +469,12 @@ def run_single_or_stripes(args, fe, rank, world, local, dev, numa):
                        "l2": "inputs (2 GiB per GPU) are larger than L2; no flush needed", "parallelism": "independent stripe per GPU" if world > 1 else "single GPU",
                        "passes_per_encode": launches / max(args.steps, 1)},
             "roofline": {"bound": "hbm", "kernel": top["kernel"], "pass": top["pass"], "achieved": top["achieved"], "peak": peak, "unit": "GB/s", "frac": top["frac"],
-                         "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src, "per_kernel": kernels,
+                         "traffic": None, "traffic_source": None, "peak_source": peak_src, "per_kernel": kernels,
                          "encode_frac_of_compulsory_bytes": round(nbytes / (ms / args.steps * 1e-3) / 1e9 / peak, 4),
                          "note": "dominant (longest) pass kernel; algorithmic bytes per launch = 2*N*SIZE*4 (one read + one write of the array per pass); "
                                  "durations = CUDA events between the launches, averaged over a loop of encodes right after the timed region"},
             "gpu_launches": int(launches),
+            "gpu": gpu_identity(local),
             "clocks": clocks,
             "parity": parity,
         }
@@ -563,6 +572,8 @@ def run_sharded(args, fe, rank, world, local, dev, numa):
     ms = multirank.max_over_ranks(ev0.elapsed_time(ev1), device=dev)
     launches = fe.kernel_launches() - launches0
     clocks = sampler.stop() if sampler else None
+    if rank == 0 and args.dump_outputs:                                 # rank 0's shard: global blocks l*G
+        dump_outputs(args.dump_outputs, x)
     sync()
     if fused:
         enc.check()                             # no barrier timed out: the ranks stayed in step
@@ -622,7 +633,7 @@ def run_sharded(args, fe, rank, world, local, dev, numa):
 
     if rank == 0:
         a2a_bytes = 2.0 * (world - 1) / world * (N * S * 4 / world)           # sent per GPU per encode (two exchanges)
-        link = 770.0                                                          # GB/s per direction per GPU, measured peer copy (B200_PROFILING.md)
+        link = 450.0                                                          # GB/s per direction per GPU: H100 SXM NVLink data sheet (900 GB/s both ways), not measured
         t_link = a2a_bytes / (link * 1e9)
         step_s = ms / args.steps * 1e-3
         out = {
@@ -640,8 +651,8 @@ def run_sharded(args, fe, rank, world, local, dev, numa):
             "roofline": {"bound": "nvlink", "kernel": "ntt_pass_kernel<9,1,2> (A) + ntt_pass_kernel<10,2,2> (BC): the instantiations whose stores pick a destination GPU",
                          "achieved": a2a_bytes / step_s / 1e9, "peak": link, "unit": "GB/s",
                          "frac": t_link / step_s, "traffic": None,
-                         "note": "bytes each GPU sends to its peers per encode (2 exchanges of (G-1)/G of the local array) / step time, against the measured 770 GB/s per-direction peer bandwidth"},
-            "gpu_launches": int(launches), "clocks": clocks, "parity": parity,
+                         "note": "bytes each GPU sends to its peers per encode (2 exchanges of (G-1)/G of the local array) / step time, against the 450 GB/s per-direction NVLink bandwidth of the H100 SXM data sheet"},
+            "gpu_launches": int(launches), "gpu": gpu_identity(local), "clocks": clocks, "parity": parity,
         }
         if phases:
             out["phases_ms_max_over_ranks"] = phases

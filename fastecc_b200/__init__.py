@@ -1,4 +1,4 @@
-"""fastecc_b200 -- B200 (sm_100a) NTT Reed-Solomon encoder behind FastECC's call surface.
+"""fastecc_b200 -- H100 (sm_90a) NTT Reed-Solomon encoder behind FastECC's call surface.
 
 Python host-side mirror of the reference interface for the one hot path (SURVEY.md section 8b):
 
@@ -7,7 +7,7 @@ Python host-side mirror of the reference interface for the one hot path (SURVEY.
     GF_Add / GF_Sub / GF_Mul / GF_Pow / GF_Root / GF_Inv  (host scalars, GF(p).cpp:37-48,110-127,254-297)
 
 Everything that computes on blocks goes through the C ABI in include/fastecc_b200.h (ctypes); there is no CPU
-fallback: if libfastecc_b200.so is missing, or no sm_100 GPU is usable, the calls raise.  `data` mirrors the
+fallback: if libfastecc_b200.so is missing, or no sm_90 GPU is usable, the calls raise.  `data` mirrors the
 reference's ``T** data``: either a C-contiguous numpy uint32 array of shape (N, SIZE) (block i = data[i]) or a
 sequence of N 1-D uint32 arrays (arbitrary block addresses).  Results are written in place.
 """

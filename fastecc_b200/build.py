@@ -1,4 +1,4 @@
-"""Build the fastecc_b200 CUDA shared library in-tree with nvcc for sm_100a (no JIT cache, no torch involved)."""
+"""Build the fastecc_b200 CUDA shared library in-tree with nvcc for sm_90a (no JIT cache, no torch involved)."""
 import os
 import subprocess
 import sys
@@ -8,7 +8,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libfastecc_b200.so")
 SOURCES = ["api.cu", "ntt_pass.cu", "small_dft.cu", "byte_recode.cu", "elementwise.cu", "decode.cu", "mixed_radix.cu"]
 HEADERS = sorted(f for f in os.listdir(CSRC) if f.endswith((".cuh", ".h"))) + [os.path.join("..", "..", "include", "fastecc_b200.h")]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC,-O3", "-shared"]
 
 

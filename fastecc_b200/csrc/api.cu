@@ -342,7 +342,7 @@ int fastecc_b200_init(int device)
     CUDA_TRY(cudaSetDevice(device));
     cudaDeviceProp prop;
     CUDA_TRY(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10) return fail(FASTECC_B200_ECUDA, "fastecc_b200_init: device %d is sm_%d%d; this library contains sm_100a code only", device, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) return fail(FASTECC_B200_ECUDA, "fastecc_b200_init: device %d is sm_%d%d; this library contains sm_90a code only", device, prop.major, prop.minor);
     Context* c = new Context;
     c->device = device; c->num_sms = prop.multiProcessorCount;
     std::vector<gf::Tw> tw(gf::M);

@@ -1,4 +1,4 @@
-// GF(0xFFF00001) arithmetic for the sm_100a NTT kernels (and a bit-identical host restatement used by the
+// GF(0xFFF00001) arithmetic for the sm_90a NTT kernels (and a bit-identical host restatement used by the
 // CPU emulation of the kernels and by the twiddle-table generator).
 //
 // Replaces, on the device, GF_Add / GF_Sub / GF_Mul of the reference (GF(p).cpp:37-48, 110-127).  The reference's
@@ -15,8 +15,8 @@
 //      addl(a, v):  a in [0,2^32), v in [0,P]  ->  a+v mod P  in [0,2^32)     (add, then +(2^32-P) on carry)
 //      subl(a, v):  a in [0,2^32), v in [0,P]  ->  a-v mod P  in [0,2^32)     (sub, then -(2^32-P) on borrow)
 // which are closed (proof in DESIGN.md section 4); canon() maps a lazy value to the canonical residue [0,P).
-// The carry idioms below compile to IADD3 Rd,Pc + @Pc VIADD (2 SASS instructions); both were validated on a B200
-// against 64-bit arithmetic (profiles/r01_ubench_int_pipes.log, "selftest" lines).
+// The carry idioms below compile to IADD3 Rd,Pc + @Pc VIADD (2 SASS instructions); tools/ubench.cu self-tests them
+// against 64-bit arithmetic on the GPU ("selftest" lines).
 #pragma once
 #include <stdint.h>
 
@@ -54,15 +54,15 @@ GF_HD uint32_t mul(uint32_t b, uint32_t w, uint32_t whi, uint32_t wlo, uint32_t 
 }
 
 // ---- the product of the pass kernels: quotient on the FP64 unit ----------------------------------------------------
-// A B200 issues IMAD.HI at half the IMAD rate (4.7 vs 2.1 cycles per warp instruction and scheduler, tools/ubench2.cu),
-// so the two IMAD.HI of mul() are 2/3 of its multiplier time.  mul_h gets the quotient from one DFMA instead:
+// IMAD.HI issues at a fraction of the IMAD rate (tools/ubench2.cu measures both), so the two IMAD.HI of mul() dominate
+// its multiplier time.  mul_h gets the quotient from one DFMA instead:
 //      wp = RD53(W * 2^-64) <= w/P                          (53-bit truncation of the same W; stage tables hold it)
 //      q  = lo32( fma.rm( double(b), wp, 2^52 ) ) = floor(b * wp)         exactly: one rounding, towards -inf, at ulp 1
 //      v  = b*w + q*(2^32-P)  (mod 2^32)                                   2 x IMAD
 // 0 <= b*(w/P - wp) < 2^32 * (2^-53 + 2^-64), so q is floor(b*w/P) or, only when (b*w mod P) <= 2^11, one less:
 // v = b*w - q*P lies in [0, P + 2^11] and fits 32 bits; one VIADDMNMX (min(v, v-P) unsigned) brings it into [0, P).
-// double(b) is an exact I2F.F64.U32.  Valid for ANY 32-bit b, like mul().  Validated on a B200 against 64-bit
-// arithmetic on 4M operand pairs incl. 1.4M adversarial ones with b*w mod P < 5000 (profiles/r02_ubench2_fp64_quotient.log).
+// double(b) is an exact I2F.F64.U32.  Valid for ANY 32-bit b, like mul().  tools/ubench2.cu checks it on the GPU against
+// 64-bit arithmetic, adversarial operands with small b*w mod P included; the CPU restatement below is tested bit for bit.
 //
 // wp_bits: the IEEE-754 encoding {lo, hi} of wp, built with integer operations only so that host and device agree.
 GF_HD uint32_t clz64(uint64_t x)
@@ -126,8 +126,8 @@ GF_HD uint32_t addl(uint32_t a, uint32_t v)
 GF_HD uint32_t subl(uint32_t a, uint32_t v)
 {
 #if defined(__CUDA_ARCH__)
-    // sub.cc leaves CF = NOT borrow for a following addc on this toolchain/hardware (checked on B200: the
-    // "subfix1" line of the self-test); so "c == 0" means a borrow happened.
+    // sub.cc leaves CF = NOT borrow for a following addc (the "subfix1" line of the tools/ubench.cu self-test);
+    // so "c == 0" means a borrow happened.
     uint32_t s;
     asm("{\n\t.reg .pred q;\n\t.reg .u32 c;\n\tsub.cc.u32 %0, %1, %2;\n\taddc.u32 c, 0, 0;\n\tsetp.eq.u32 q, c, 0;\n\t@q sub.u32 %0, %0, 0xFFFFF;\n\t}"
         : "=r"(s) : "r"(a), "r"(v));

@@ -1,4 +1,4 @@
-// The sm_100a pass kernel: one launch = one pass of the four-step / MFA decomposition (MFA_NTT, ntt.cpp:382-447)
+// The sm_90a pass kernel: one launch = one pass of the four-step / MFA decomposition (MFA_NTT, ntt.cpp:382-447)
 // over the whole [N][SIZE] array, or -- with two transforms fused on a tile -- the end of the inverse transform,
 // the RS scaling (RS.cpp:51-59) and the start of the forward transform in a single pass.
 //
@@ -12,7 +12,7 @@
 //   * ceil(LR/5) <= 2 register rounds of up to five radix-2 stages (three for a fused two-transform tile, whose
 //     middle round runs 4+5 stages back to back in registers) separated by one block barrier each;
 //   * 64-bit stores of the finished rows straight from registers.
-// The kernel is bound by instruction issue (XU conversions + FP64 / integer multiplies + the lazy add/sub), not by HBM: see profiles/.
+// The kernel is bound by instruction issue (XU conversions + FP64 / integer multiplies + the lazy add/sub), not by HBM: DESIGN.md section 6.
 #include "ntt_tile.cuh"
 #include "ntt_pass.h"
 #include "plan.h"
@@ -81,11 +81,11 @@ __global__ void __launch_bounds__(kThreads, 2) ntt_pass_kernel(const PassParams 
     uint4* tile = smem;                                   // 4096 chunks, natural row order
     // stage tables: a transform whose twist does not depend on the row set (t1 == 0) has ONE table, loaded once;
     // the others are double-buffered per set.  Slot of transform x in buffer b: tabs + (b*NXF + x)*R; set-independent
-    // tables always use b = 0 (so a fused BC tile needs 3 slots, a plain A tile 1).
-    uint4* tabs = smem + kTileChunks;
+    // tables always use b = 0 (so a fused BC tile needs 3 slots, a plain A tile 1).  The two mbarriers sit between the
+    // tile and the tables, at an address known at compile time (one register fewer to keep live across the tile loop).
+    uint64_t* bar = reinterpret_cast<uint64_t*>(smem + kTileChunks);
+    uint4* tabs = smem + kTileChunks + 1;
     const bool var0 = P.xf[0].t1 != 0, var1 = NXF == 2 && P.xf[1].t1 != 0;
-    const uint32_t nslots = var1 ? 4u : (var0 ? (uint32_t)NXF + 1u : (uint32_t)NXF);
-    uint64_t* bar = reinterpret_cast<uint64_t*>(tabs + nslots * R);
     const uint32_t tid  = threadIdx.x;
     const uint32_t groups = (P.nstrips + P.strips_per_item - 1) / P.strips_per_item;
     const uint32_t nitems = P.nsets * groups;
@@ -198,11 +198,11 @@ cudaError_t launch_build_tables(PassParams& P, uint4* out, cudaStream_t stream)
     const uint32_t ns = table_sets(P);
     P.tables = out;
     P.table_set_stride = ns > 1 ? (P.nxf << P.log_r) : 0u;
-    build_tables_kernel<<<592, 256, 0, stream>>>(P, out, ns);
+    build_tables_kernel<<<528, 256, 0, stream>>>(P, out, ns);        // 4 CTAs per SM of an H100 (132 SMs), grid-stride
     return cudaGetLastError();
 }
 
-// shared memory of the CTA-level kernel: tile + table slots + two mbarriers.  Table slot of transform x in buffer b is
+// shared memory of the CTA-level kernel: tile + two mbarriers + table slots.  Table slot of transform x in buffer b is
 // (b*nxf + x); buffer 1 is needed only up to the last set-dependent transform.
 size_t pass_smem_bytes(const PassParams& P)
 {

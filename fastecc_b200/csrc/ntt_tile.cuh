@@ -1,6 +1,6 @@
 // Tile-level decimation-in-time NTT over GF(0xFFF00001): the code every pass kernel runs per 64 KiB tile.
 //
-// This header is the B200 counterpart of the reference's inner loops
+// This header is the GPU counterpart of the reference's inner loops
 //     IterativeNTT_Steps  ntt.cpp:251-284   (radix-2 butterflies across blocks, inner loop over the SIZE words)
 //     revbin_permute      ntt.cpp:292-309   (here: bit-reversed *addressing* when a tile is loaded, no data pass)
 //     MFA twiddle loop    ntt.cpp:421-431   (here: folded into the butterfly twiddles of the next pass, see below)
@@ -198,6 +198,28 @@ FECC_HD RoundCtx make_round(uint32_t LR, uint32_t k, uint32_t j)
 
 struct RoundRegs { uint2 x[kRows]; };
 
+// Stage BETA of a round (pairs differing in in-thread bit BETA).  BETA is a template parameter so that both loops have
+// compile-time trip counts: for sm_90a the front end leaves a loop of (16 >> beta) trips rolled when beta comes from an
+// enclosing unrolled loop, and the 32 slots then live in local memory instead of registers.
+template <bool BREV, int BETA>
+FECC_HD void stage_compute(uint2 (&x)[kRows], const RoundCtx& c, const uint4* tb, uint32_t sb)
+{
+    const uint32_t b = c.lb + BETA;
+    if (b >= c.blo && b < c.bhi) {
+        const uint4* twp = tb + (sb << BETA);           // heap entry 2^b + jlow (+ m * 2^lb)
+#pragma unroll
+        for (int m = 0; m < (1 << BETA); ++m) {
+            const uint4 w = *twp; twp += sb;
+#pragma unroll
+            for (int hi = 0; hi < (16 >> BETA); ++hi) {
+                const int i0 = (hi << (BETA + 1)) | m;
+                const int i1 = i0 | (1 << BETA);
+                bfly2(x[BREV ? brev5(i0) : i0], x[BREV ? brev5(i1) : i1], w);
+            }
+        }
+    }
+}
+
 // Up to five radix-2 DIT stages on the thread's 32 slots x 2 words.  tw points at the heap-ordered stage table of the
 // current transform (shared memory on the device).  BREV: the registers are numbered in the order of the PREVIOUS
 // transform's last round (fused tiles): this transform's slot i is register brev5(i).
@@ -206,20 +228,28 @@ FECC_HD void round_compute(uint2 (&x)[kRows], const RoundCtx& c, const uint4* tw
 {
     const uint32_t sb = 1u << c.lb;                     // table stride between consecutive in-thread twiddles
     const uint4* tb = tw + c.jlow;
+    stage_compute<BREV, 0>(x, c, tb, sb);
+    stage_compute<BREV, 1>(x, c, tb, sb);
+    stage_compute<BREV, 2>(x, c, tb, sb);
+    stage_compute<BREV, 3>(x, c, tb, sb);
+    stage_compute<BREV, 4>(x, c, tb, sb);
+}
+
+// Stage BETA >= 1 of round0_plain (compile-time BETA for the reason given at stage_compute)
+template <int BETA>
+FECC_HD void stage0_plain(uint2 (&x)[kRows], const RoundCtx& c, const uint4* tw)
+{
+    if ((uint32_t)BETA < c.bhi) {
+        const uint4* twb = tw + (1u << BETA);
 #pragma unroll
-    for (int beta = 0; beta < kStages; ++beta) {
-        const uint32_t b = c.lb + beta;
-        if (b >= c.blo && b < c.bhi) {
-            const uint4* twp = tb + (sb << beta);       // heap entry 2^b + jlow (+ m * 2^lb)
+        for (int m = 0; m < (1 << BETA); ++m) {
+            uint4 w = {0, 0, 0, 0};
+            if (m) w = twb[m];
 #pragma unroll
-            for (int m = 0; m < (1 << beta); ++m) {
-                const uint4 w = *twp; twp += sb;
-#pragma unroll
-                for (int hi = 0; hi < (16 >> beta); ++hi) {
-                    const int i0 = (hi << (beta + 1)) | m;
-                    const int i1 = i0 | (1 << beta);
-                    bfly2(x[BREV ? brev5(i0) : i0], x[BREV ? brev5(i1) : i1], w);
-                }
+            for (int hi = 0; hi < (16 >> BETA); ++hi) {
+                const int i0 = (hi << (BETA + 1)) | m;
+                const int i1 = i0 | (1 << BETA);
+                if (m) bfly2(x[i0], x[i1], w); else bfly2_trivial(x[i0], x[i1]);
             }
         }
     }
@@ -244,23 +274,10 @@ FECC_HD void round0_plain(uint2 (&x)[kRows], const RoundCtx& c, const uint4* tw,
             bfly2_trivial(a, b);
         }
     }
-#pragma unroll
-    for (int beta = 1; beta < kStages; ++beta) {
-        if ((uint32_t)beta < c.bhi) {
-            const uint4* twb = tw + (1u << beta);
-#pragma unroll
-            for (int m = 0; m < (1 << beta); ++m) {
-                uint4 w = {0, 0, 0, 0};
-                if (m) w = twb[m];
-#pragma unroll
-                for (int hi = 0; hi < (16 >> beta); ++hi) {
-                    const int i0 = (hi << (beta + 1)) | m;
-                    const int i1 = i0 | (1 << beta);
-                    if (m) bfly2(x[i0], x[i1], w); else bfly2_trivial(x[i0], x[i1]);
-                }
-            }
-        }
-    }
+    stage0_plain<1>(x, c, tw);
+    stage0_plain<2>(x, c, tw);
+    stage0_plain<3>(x, c, tw);
+    stage0_plain<4>(x, c, tw);
 }
 
 FECC_HD void prescale_all(uint2 (&x)[kRows], uint32_t w, uint32_t wp_lo, uint32_t wp_hi)

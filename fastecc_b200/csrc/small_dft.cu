@@ -58,7 +58,7 @@ cudaError_t launch_small_dft(uint32_t* data, uint32_t pitch4, uint32_t s4, uint3
     return cudaGetLastError();
 }
 
-// [N][size] with arbitrary pitch/alignment  <->  [N][pitch4*4] 16-byte aligned, pad words zero
+// [N][size] with arbitrary pitch/alignment  <->  [N][pitch4*4] 16-byte aligned, pad words zero (grid-stride; 8 CTAs per SM of an H100)
 __global__ void repack_kernel(const uint32_t* src, size_t src_pitch, uint32_t* dst, size_t dst_pitch,
                               size_t n_rows, uint32_t size, uint32_t copy_cols, uint32_t zero_from)
 {
@@ -71,13 +71,13 @@ __global__ void repack_kernel(const uint32_t* src, size_t src_pitch, uint32_t* d
 cudaError_t launch_pack(const uint32_t* src, size_t src_pitch, uint32_t* dst, size_t dst_pitch, size_t n_rows,
                         uint32_t size, cudaStream_t stream)
 {
-    repack_kernel<<<1184, 256, 0, stream>>>(src, src_pitch, dst, dst_pitch, n_rows, size, (uint32_t)dst_pitch, size);
+    repack_kernel<<<1056, 256, 0, stream>>>(src, src_pitch, dst, dst_pitch, n_rows, size, (uint32_t)dst_pitch, size);
     return cudaGetLastError();
 }
 cudaError_t launch_unpack(const uint32_t* src, size_t src_pitch, uint32_t* dst, size_t dst_pitch, size_t n_rows,
                           uint32_t size, cudaStream_t stream)
 {
-    repack_kernel<<<1184, 256, 0, stream>>>(src, src_pitch, dst, dst_pitch, n_rows, size, size, size);
+    repack_kernel<<<1056, 256, 0, stream>>>(src, src_pitch, dst, dst_pitch, n_rows, size, size, size);
     return cudaGetLastError();
 }
 

@@ -1,5 +1,5 @@
 // Drop-in replacement for the reference's ntt.cpp: lets the UNMODIFIED reference drivers (main.cpp -> `ntt`,
-// RS.cpp -> `rs`) run their GF(0xFFF00001) transforms on the B200 through the C ABI of include/fastecc_b200.h.
+// RS.cpp -> `rs`) run their GF(0xFFF00001) transforms on the H100 through the C ABI of include/fastecc_b200.h.
 //
 // The reference programs textually `#include "ntt.cpp"` (main.cpp:18, RS.cpp:18).  integration/build_dropin.sh builds
 // them from a staging directory that holds symlinks to the reference sources plus THIS file under the name ntt.cpp,
@@ -28,7 +28,7 @@ void MFA_NTT (T** data, size_t N, size_t SIZE, bool InvNTT)
     MFA_NTT_reference_cpu<T,P> (data, N, SIZE, InvNTT);
 }
 
-// GF(0xFFF00001): the B200
+// GF(0xFFF00001): the H100
 template <>
 inline void MFA_NTT<uint32_t,0xFFF00001> (uint32_t** data, size_t N, size_t SIZE, bool InvNTT)
 {

@@ -1,4 +1,4 @@
-/* fastecc_b200 -- C ABI of the B200 (sm_100a) NTT Reed-Solomon encoder.
+/* fastecc_b200 -- C ABI of the H100 (sm_90a) NTT Reed-Solomon encoder.
  *
  * This is the drop-in boundary for the one hot path of Bulat-Ziganshin/FastECC.  The reference has no FFI layer:
  * its programs textually include the template sources, so the boundary is created at the narrowest existing call

@@ -1,5 +1,5 @@
 #!/bin/bash
-# Builds the reference's own drivers (main.cpp -> ntt-b200, RS.cpp -> rs-b200) UNMODIFIED against the B200 library.
+# Builds the reference's own drivers (main.cpp -> ntt-b200, RS.cpp -> rs-b200) UNMODIFIED against the H100 library.
 # Needs the reference tree (default /root/reference); outputs go to oracle/_ref/dropin/ (git-ignored, travels to
 # the GPU box with gpurun).  Nothing from the reference is copied: the staging directory only holds symlinks.
 set -euo pipefail

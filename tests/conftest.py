@@ -10,7 +10,7 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run on the GPU box with `-m gpu`)")
+    config.addinivalue_line("markers", "gpu: needs a real H100 (run on a GPU machine with `-m gpu`)")
 
 
 @pytest.fixture(scope="session")

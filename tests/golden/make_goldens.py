@@ -1,7 +1,9 @@
-"""Regenerates / cross-checks tests/golden/survey_8c.json against the reference compiled in oracle/_ref.
+"""Regenerates / cross-checks tests/golden/survey_8c.json, vectors.npz and reference_cross.json against the reference
+compiled in oracle/_ref.
 
-Needs /root/reference (this container only).  Usage: python tests/golden/make_goldens.py [--write]
-Without --write it only verifies that the committed file matches what the reference computes here.
+Needs oracle/_ref built from a reference tree (oracle/Makefile, REF=<path>).  Usage: python tests/golden/make_goldens.py [--write]
+--write rewrites vectors.npz and reference_cross.json; without it the committed files are only verified against what the
+reference computes here.
 """
 import json
 import os
@@ -16,7 +18,7 @@ import oracle_lib as ol  # noqa: E402
 
 def main():
     o, r = ol.load_oracle(), ol.load_ref()
-    assert r is not None, "oracle/_ref/libfastecc_ref.so missing (needs /root/reference)"
+    assert r is not None, "oracle/_ref/libfastecc_ref.so missing (build it from a reference tree: make -C oracle REF=<path>)"
     g = json.load(open(os.path.join(HERE, "survey_8c.json")))
     bad = 0
 
@@ -55,16 +57,27 @@ def main():
         for inv in (0, 1):
             y = x.copy(); r.ref_mfa_ntt_flat(y.ctypes.data, N, S, inv); vec["ntt%d_%d_%d" % (inv, L, S)] = y
         y = x.copy(); r.ref_rs_encode_flat(y.ctypes.data, N, S); vec["enc_%d_%d" % (L, S)] = y
+    # the reference's results on the inputs of tests/test_oracle.py::test_against_compiled_reference
+    def ref_ntt(a, inv):
+        b = a.copy(); r.ref_mfa_ntt_flat(b.ctypes.data, b.shape[0], b.shape[1], inv); return b
+
+    def ref_encode(a):
+        b = a.copy(); r.ref_rs_encode_flat(b.ctypes.data, b.shape[0], b.shape[1]); return b
+    cross = ol.cross_record(o, lambda x, y: (r.ref_gf_mul(x, y), r.ref_gf_add(x, y), r.ref_gf_sub(x, y)), ref_ntt, ref_encode)
     path = os.path.join(HERE, "vectors.npz")
+    cross_path = os.path.join(HERE, "reference_cross.json")
     if "--write" in sys.argv:
         np.savez_compressed(path, **vec)
-        print("wrote", path)
+        with open(cross_path, "w") as f:
+            json.dump(cross, f, separators=(",", ":"))
+        print("wrote", path, cross_path)
     else:
         old = np.load(path)
         for k, v in vec.items():
             if not np.array_equal(old[k], v):
                 bad += 1
                 print("MISMATCH vector", k)
+        chk("reference_cross.json", json.load(open(cross_path)), cross)
     print("goldens", "MISMATCH" if bad else "verified against the compiled reference")
     return 1 if bad else 0
 

@@ -80,3 +80,24 @@ def o_encode(o, a):
     b = np.ascontiguousarray(a).copy()
     assert o.oracle_rs_encode(b.ctypes.data, b.shape[0], b.shape[1]) == 0
     return b
+
+
+CROSS_SHAPES = ((2, 3), (6, 17), (9, 1024), (10, 16), (11, 64), (13, 33))     # (log2 N, SIZE): flat / 2-D / cube paths of MFA_NTT
+
+
+def cross_record(o, gf, ntt, encode):
+    """gf(x, y) -> (mul, add, sub) on 200 seeded pairs, and SHA-256 digests of ntt(a, inverse) and encode(a) on fill B of
+    every CROSS_SHAPES entry.  Recorded from the compiled reference by tests/golden/make_goldens.py into
+    tests/golden/reference_cross.json; tests/test_oracle.py recomputes it with the oracle."""
+    import hashlib
+    rng = np.random.default_rng(3)
+    rec = {"gf": [], "digests": {}}
+    for _ in range(200):
+        x, y = int(rng.integers(0, P)), int(rng.integers(0, P))
+        rec["gf"].append([x, y] + [int(v) for v in gf(x, y)])
+    for L, S in CROSS_SHAPES:
+        a = fill_B(o, 1 << L, S)
+        for inv in (0, 1):
+            rec["digests"]["ntt%d_%d_%d" % (inv, L, S)] = hashlib.sha256(ntt(a, inv).tobytes()).hexdigest()
+        rec["digests"]["enc_%d_%d" % (L, S)] = hashlib.sha256(encode(a).tobytes()).hexdigest()
+    return rec

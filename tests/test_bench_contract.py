@@ -1,5 +1,5 @@
 """bench.py contract on the CPU: the reference arm (the only arm that runs without a GPU) prints exactly ONE JSON line
-on stdout with the keys the driver reads; non-zero ranks of a torchrun launch stay silent; the B200 arm fails loudly
+on stdout with the keys the driver reads; non-zero ranks of a torchrun launch stay silent; the GPU arm fails loudly
 (no JSON, non-zero exit) when there is no CUDA device -- there is no CPU fallback to fall into."""
 import json
 import os

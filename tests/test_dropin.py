@@ -1,4 +1,4 @@
-"""The reference's own drivers, UNMODIFIED, built against the B200 library through fastecc_b200/shim/ntt.cpp.
+"""The reference's own drivers, UNMODIFIED, built against the H100 library through fastecc_b200/shim/ntt.cpp.
 
 CPU part: the shim compiles and links (only where the reference tree exists).  GPU part: `ntt-b200 n L 4096` -- the
 reference's integration test of MFA_NTT (main.cpp:239-300: forward, inverse, x N^-1, hashes) -- must print

@@ -1,5 +1,5 @@
 """CPU: the built library really contains what DESIGN.md says the kernels are made of.  cuobjdump -sass of
-fastecc_b200/libfastecc_b200.so (sm_100a cubins only): the headline pass kernels take their quotient from the FP64 unit
+fastecc_b200/libfastecc_b200.so (sm_90a cubins only): the headline pass kernels take their quotient from the FP64 unit
 (I2F.F64.U32 + DFMA.RM + VIADDMNMX.U32, one each per product, and no IMAD.HI in the butterflies), load their tiles and tables
 with TMA (UTMALDG / UBLKCP + SYNCS mbarrier instructions) and do not spill."""
 import os
@@ -19,7 +19,7 @@ def sass():
     if not os.path.exists(exe) or not os.path.exists(LIB):
         pytest.skip("needs cuobjdump and the built library")
     elf = subprocess.run([exe, "-lelf", LIB], capture_output=True, text=True, check=True).stdout
-    assert "sm_100a" in elf and not re.search(r"sm_(?!100a)\d+", elf), elf
+    assert "sm_90a" in elf and not re.search(r"sm_(?!90a)\d+", elf), elf
     out = subprocess.run([exe, "-sass", LIB], capture_output=True, text=True, check=True).stdout
     kernels, name = {}, None
     for line in out.splitlines():

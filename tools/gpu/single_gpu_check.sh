@@ -1,7 +1,6 @@
 #!/bin/bash
-# Everything measured on ONE B200, in the order the driver runs it plus the profiling passes.  Run from the repo root under gpurun
-# (about 6 minutes):  gpurun --timeout 2400 -- 'bash tools/gpu/single_gpu_check.sh'.  Outputs land in gpurun_out/; copy what
-# should be judged into profiles/.
+# Everything measured on ONE H100, in the order the driver runs it plus the profiling passes.  Run from the repo root
+# (about 6 minutes); outputs land in the directory created below.
 mkdir -p gpurun_out
 timeout 1200 python -m pytest tests -x -q -m gpu 2>&1 | tail -4 | tee gpurun_out/pytest_gpu.log
 timeout 200 python -c "import __graft_entry__ as g; g.smoke()" 2>&1 | tail -2

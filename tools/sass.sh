@@ -4,7 +4,7 @@
 cd "$(dirname "$0")/.."
 LIB=${1:-fastecc_b200/libfastecc_b200.so}
 cuobjdump -sass $LIB > /tmp/all.sass
-echo "# $LIB  ($(cuobjdump -lelf $LIB | grep -c sm_100a) sm_100a cubins)"
+echo "# $LIB  ($(cuobjdump -lelf $LIB | grep -c sm_90a) sm_90a cubins)"
 for pat in "pass_kernelILi10ELi2ELi1" "pass_kernelILi9ELi1ELi1" "pass_kernelILi9ELi1ELi2" "pass_kernelILi10ELi2ELi2"; do
   s=$(grep -n "Function : .*${pat}" /tmp/all.sass | cut -d: -f1)
   [ -z "$s" ] && continue

@@ -1,4 +1,4 @@
-// Micro-benchmarks + primitive self-tests for GF(0xFFF00001) on sm_100a.  Scratch tool (not product).
+// Micro-benchmarks + primitive self-tests for GF(0xFFF00001) on sm_90a.  Scratch tool (not product).
 #include <cstdio>
 #include <cstdint>
 #include <cstdlib>

@@ -1,4 +1,4 @@
-// Micro-benchmark: can the FP64 pipe of a B200 take the quotient of the GF(0xFFF00001) constant product off the integer
+// Micro-benchmark: can the FP64 pipe of the GPU take the quotient of the GF(0xFFF00001) constant product off the integer
 // multiplier?  (VERDICT r01 "Next" #2.)  Scratch tool, not product.
 //
 //   Barrett (production r01):  q = hi32(b*Whi + hi32(b*Wlo))                        2 x IMAD.HI (4.3 cyc each, fmaheavy)
