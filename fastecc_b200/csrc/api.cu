@@ -10,13 +10,26 @@
 #include <cstdio>
 #include <cstdarg>
 #include <cstring>
-#include <cstdlib>
 #include <mutex>
 #include <vector>
 #include <atomic>
 #include <map>
+#include <tuple>
 
 using namespace fecc;
+
+namespace {
+thread_local char g_err[512] = "no error";
+}
+
+namespace fecc {
+// Records the message for fastecc_b200_last_error() (per thread) and returns `code`; shared with decode.cu.
+int fail(int code, const char* fmt, ...)
+{
+    va_list ap; va_start(ap, fmt); vsnprintf(g_err, sizeof g_err, fmt, ap); va_end(ap);
+    return code;
+}
+}
 
 namespace {
 
@@ -32,30 +45,50 @@ struct DevBuf {
     void release() { if (p) cudaFree(p); p = nullptr; bytes = 0; }
 };
 
-// Stage tables of one plan: built once, on the stream of the first call that needs them.  `ready` is recorded behind the
+// Stage tables of one pass: built once, on the stream of the first call that needs them.  `ready` is recorded behind the
 // build; a call on any other stream waits for it (a no-op once the build has finished).
-struct TableSet {
-    struct Slot { DevBuf buf; cudaEvent_t ready = nullptr; cudaStream_t built_on = nullptr; };
-    std::vector<Slot> slots;             // one block per pass (plan.h table_bytes)
+struct TableSlot { DevBuf buf; cudaEvent_t ready = nullptr; cudaStream_t built_on = nullptr; };
+enum Kind { kNtt, kEncode, kEncodeAsym, kShard, kShardP2P, kNttShardP2P };
+struct TableKey {                        // what the stage tables of a plan depend on
+    int kind, inverse, n_ranks, rank;
+    int sub;                             // which pass of a sharded plan, or log2(N / M) of an asymmetric encode
+    int log_n;
+    bool operator<(const TableKey& o) const
+    { return std::tie(kind, inverse, n_ranks, rank, sub, log_n) < std::tie(o.kind, o.inverse, o.n_ranks, o.rank, o.sub, o.log_n); }
 };
-// A buffer shared by calls that may come in on different streams (the Y buffer of the two-pass NTT, the repack buffer):
-// `done` is recorded behind its last use and the next user on another stream waits for it, so that two transforms in
-// flight on two streams are serialised on the buffer instead of racing on it.
+
+// A buffer shared by calls that may come in on different threads and streams (the Y buffer of the two-pass NTT, the repack
+// buffer, the destination of the order-3 / order-9 step).  Only a Lease touches it.
 struct SharedBuf {
+    std::mutex mu;
     DevBuf buf;
-    cudaEvent_t done = nullptr;
+    cudaEvent_t done = nullptr;          // recorded behind the last lease's launches
     cudaStream_t last = nullptr;
     bool used = false;
-    cudaError_t acquire(size_t need, cudaStream_t st) {
-        if (need > buf.bytes && used) { cudaError_t e = cudaEventSynchronize(done); if (e != cudaSuccess) return e; }     // about to be reallocated
-        cudaError_t e = buf.reserve(need);
-        if (e != cudaSuccess) return e;
-        if (!done) { e = cudaEventCreateWithFlags(&done, cudaEventDisableTiming); if (e != cudaSuccess) return e; }
-        if (used && last != st) e = cudaStreamWaitEvent(st, done, 0);
+    void destroy() { buf.release(); if (done) cudaEventDestroy(done); done = nullptr; used = false; }
+};
+// Exclusive use of a SharedBuf for the launches of one call: the buffer's mutex is held from construction to destruction,
+// and the destructor records `done` on the caller's stream on every exit path, error returns included.  A user on another
+// stream waits for `done` in acquire(), so two transforms that need the same buffer run one after the other on the device
+// and the buffer is never reallocated under launches that still use it.
+// Lock order: g_host_mu -> packed -> (scratch | mixed, never both at once) -> g_mu.
+class Lease {
+public:
+    Lease(SharedBuf* s, cudaStream_t st) : s_(s), st_(st) { if (s_) lk_ = std::unique_lock<std::mutex>(s_->mu); }
+    ~Lease() { if (s_ && s_->done) { s_->used = true; s_->last = st_; cudaEventRecord(s_->done, st_); } }
+    cudaError_t acquire(size_t need)
+    {
+        if (need > s_->buf.bytes && s_->used) { cudaError_t e = cudaEventSynchronize(s_->done); if (e != cudaSuccess) return e; }   // about to be reallocated
+        cudaError_t e = s_->buf.reserve(need);
+        if (e == cudaSuccess && !s_->done) e = cudaEventCreateWithFlags(&s_->done, cudaEventDisableTiming);
+        if (e == cudaSuccess && s_->used && s_->last != st_) e = cudaStreamWaitEvent(st_, s_->done, 0);
         return e;
     }
-    cudaError_t release_to(cudaStream_t st) { used = true; last = st; return cudaEventRecord(done, st); }
-    void destroy() { buf.release(); if (done) cudaEventDestroy(done); done = nullptr; used = false; }
+    uint32_t* ptr() const { return s_ ? (uint32_t*)s_->buf.p : nullptr; }
+private:
+    SharedBuf* s_;
+    cudaStream_t st_;
+    std::unique_lock<std::mutex> lk_;
 };
 
 struct Context {
@@ -65,8 +98,8 @@ struct Context {
     SharedBuf scratch;   // Y buffer of the two-pass NTT and of the asymmetric encode
     SharedBuf packed;    // repacked copy for unaligned device layouts
     SharedBuf mixed;     // destination of the order-3 / order-9 step of the N = 3 * 2^k, 9 * 2^k transforms
-    DevBuf staging;      // device copy for the host (T**) entry points (serialised by g_mu)
-    std::map<uint32_t, TableSet> tables;              // per (mode, log2 N, ...)
+    DevBuf staging;      // device copy for the host (T**) entry points (serialised by g_host_mu)
+    std::map<TableKey, std::vector<TableSlot>> tables;   // one slot per pass of the plan
     bool pin_caller = false;                          // fastecc_b200_pin_host_buffers()
     std::vector<std::pair<char*, size_t>> registered; // caller buffers we page-locked in place (cudaHostRegister)
     cudaStream_t stream = nullptr;       // compute
@@ -75,18 +108,19 @@ struct Context {
 };
 
 Context* g_ctx = nullptr;
-std::mutex g_mu;          // guards g_ctx, the table cache and the shared buffers' bookkeeping (short critical sections)
+std::mutex g_mu;          // guards g_ctx and the table cache (short critical sections)
 std::mutex g_host_mu;     // held by the host (T**) entry points for their whole duration: they share the staging buffer, three streams and the chunk events
 std::atomic<unsigned long long> g_launches{0};
-thread_local char g_err[512] = "no error";
 
-int fail(int code, const char* fmt, ...)
-{
-    va_list ap; va_start(ap, fmt); vsnprintf(g_err, sizeof g_err, fmt, ap); va_end(ap);
-    return code;
-}
 #define CUDA_TRY(expr) do { cudaError_t e_ = (expr); if (e_ != cudaSuccess) \
     return fail(e_ == cudaErrorMemoryAllocation ? FASTECC_B200_ENOMEM : FASTECC_B200_ECUDA, "%s: %s", #expr, cudaGetErrorString(e_)); } while (0)
+
+// The live context, or nullptr after recording the ENOINIT message.
+Context* ctx(const char* who)
+{
+    if (!g_ctx) fail(FASTECC_B200_ENOINIT, "%s: call fastecc_b200_init() first", who);
+    return g_ctx;
+}
 
 // N = r * 2^k with r = 3 or 9: the orders served by mixed_radix.cu on top of the power-of-two kernels (transforms only)
 uint32_t odd_factor(size_t N)
@@ -95,17 +129,31 @@ uint32_t odd_factor(size_t N)
     while (!(N & 1)) N >>= 1;
     return (uint32_t)(N <= 9 ? N : 0);
 }
+constexpr size_t kMaxPitch = 0xFFFFFFF0u;
 int check_shape(size_t N, size_t size, size_t max_log, const char* who, bool allow_mixed = false)
 {
-    if (size == 0) return fail(FASTECC_B200_EINVAL, "%s: SIZE must be >= 1 word", who);
+    if (size == 0 || size > kMaxPitch) return fail(FASTECC_B200_EINVAL, "%s: SIZE_words=%zu must be in [1, 2^32 - 16]", who, size);
     const uint32_t r = odd_factor(N);
-    if (allow_mixed && (r == 3 || r == 9) && is_pow2(N / r) && N / r <= ((size_t)1 << max_log)) {
-        if (size > 0xFFFFFFF0u) return fail(FASTECC_B200_EINVAL, "%s: SIZE too large", who);
-        return 0;
-    }
-    if (!is_pow2(N) || N > ((size_t)1 << max_log))
+    const size_t pow2_part = allow_mixed && (r == 3 || r == 9) ? N / r : N;
+    if (!is_pow2(pow2_part) || pow2_part > ((size_t)1 << max_log))
         return fail(FASTECC_B200_EINVAL, "%s: N=%zu must be a power of two in [1, 2^%zu]%s (P-1 = 2^20*4095)", who, N, max_log, allow_mixed ? ", or 3 or 9 times one" : "");
-    if (size > 0xFFFFFFF0u) return fail(FASTECC_B200_EINVAL, "%s: SIZE too large", who);
+    return 0;
+}
+int check_asym_shape(size_t N, size_t M, size_t size, const char* who)
+{
+    if (int rc = check_shape(N, size, FASTECC_B200_MAX_LOG_N_ENCODE, who)) return rc;
+    if (!is_pow2(M) || M > N) return fail(FASTECC_B200_EINVAL, "%s: M=%zu must be a power of two in [1, N]", who, M);
+    return 0;
+}
+// A device buffer of `rows` rows of `pitch` words, the first SIZE of each meaningful: d != null, 1 <= SIZE <= pitch <= 2^32 - 16,
+// fewer than 2^32 16-byte chunks (the kernels index them in 32 bits); `aligned`: pitch % 4 == 0 and d 16-byte aligned as well.
+int check_rows(const void* d, size_t rows, size_t size, size_t pitch, bool aligned, const char* who)
+{
+    if (!d) return fail(FASTECC_B200_EINVAL, "%s: null device pointer", who);
+    if (size == 0 || pitch < size || pitch > kMaxPitch) return fail(FASTECC_B200_EINVAL, "%s: needs 1 <= SIZE_words (%zu) <= pitch_words (%zu) <= 2^32 - 16", who, size, pitch);
+    if (aligned && (pitch % 4 || (uintptr_t)d % 16)) return fail(FASTECC_B200_EINVAL, "%s: needs pitch_words %% 4 == 0 and a 16-byte aligned buffer", who);
+    if ((unsigned long long)rows * ((pitch + 3) / 4) >= (1ull << 32))
+        return fail(FASTECC_B200_EINVAL, "%s: buffer of %zu x %zu words is 64 GiB or more (32-bit chunk indexing)", who, rows, pitch);
     return 0;
 }
 
@@ -129,16 +177,15 @@ void pin_caller_array(Context* c, void* base, size_t bytes)
     else cudaGetLastError();
 }
 
-// Stage tables of `plan` under cache key `key`: built on first use (into a local set that enters the cache only when every
-// block is allocated and its build launched), then attached to the passes.  which >= 0: only that pass of a 3-pass plan.
-int attach_tables(Context* c, uint32_t key, std::vector<PassParams>& plan, cudaStream_t st, int which = -1, size_t slots = 0)
+// Stage tables of `plan` under cache key `key`: built on first use (a block enters the cache only once it is allocated and
+// its build launched), then attached to the passes.
+int attach_tables(Context* c, const TableKey& key, std::vector<PassParams>& plan, cudaStream_t st)
 {
     std::lock_guard<std::mutex> lk(g_mu);
-    TableSet& ts = c->tables[key];
-    const size_t n = slots ? slots : plan.size();
-    if (ts.slots.size() != n) ts.slots.resize(n);
+    std::vector<TableSlot>& slots = c->tables[key];
+    slots.resize(plan.size());
     for (size_t i = 0; i < plan.size(); ++i) {
-        TableSet::Slot& sl = ts.slots[which >= 0 ? (size_t)which : i];
+        TableSlot& sl = slots[i];
         if (!sl.buf.p) {
             DevBuf nb;
             cudaEvent_t ev = nullptr;
@@ -185,11 +232,10 @@ int run_aligned(Context* c, uint32_t* x, size_t N, size_t size, size_t pitch, in
         if (M > 1)                                        // step 1: r transforms of order M, each on every r-th row (row pitch r times larger), in place
             for (uint32_t n1 = 0; n1 < r; ++n1)
                 if (int rc = run_aligned(c, x + (size_t)n1 * pitch, M, size, (size_t)r * pitch, mode, st)) return rc;
-        { std::lock_guard<std::mutex> lk(g_mu); CUDA_TRY(c->mixed.acquire(N * pitch * sizeof(uint32_t), st)); }
-        uint32_t* y = (uint32_t*)c->mixed.buf.p;          // step 2: twiddles + order-r transform, into natural order (out of place), then back
-        CUDA_TRY(launch_radix_pass(x, y, pitch4, s4, r, (uint32_t)M, mode == 1, c->d_tw, c->num_sms, st)); g_launches++;
-        CUDA_TRY(cudaMemcpy2DAsync(x, pitch * 4, y, pitch * 4, (size_t)s4 * 16 < pitch * 4 ? (size_t)s4 * 16 : pitch * 4, N, cudaMemcpyDeviceToDevice, st));
-        { std::lock_guard<std::mutex> lk(g_mu); CUDA_TRY(c->mixed.release_to(st)); }
+        Lease y(&c->mixed, st);                           // step 2: twiddles + order-r transform, into natural order (out of place), then back
+        CUDA_TRY(y.acquire(N * pitch * sizeof(uint32_t)));
+        CUDA_TRY(launch_radix_pass(x, y.ptr(), pitch4, s4, r, (uint32_t)M, mode == 1, c->d_tw, c->num_sms, st)); g_launches++;
+        CUDA_TRY(cudaMemcpy2DAsync(x, pitch * 4, y.ptr(), pitch * 4, (size_t)s4 * 16 < pitch * 4 ? (size_t)s4 * 16 : pitch * 4, N, cudaMemcpyDeviceToDevice, st));
         return 0;
     }
     if (N < ((size_t)1 << kMinLogR)) {
@@ -200,18 +246,13 @@ int run_aligned(Context* c, uint32_t* x, size_t N, size_t size, size_t pitch, in
         g_launches++;
         return 0;
     }
-    Buffers b{x, nullptr, c->d_tw, (uint32_t)pitch, (uint32_t)size};
     const bool need_y = mode != 2 && !single_pass(ilog2(N));               // the two-pass NTT ping-pongs through Y
-    if (need_y) {
-        std::lock_guard<std::mutex> lk(g_mu);
-        CUDA_TRY(c->scratch.acquire(N * pitch * sizeof(uint32_t), st));
-        b.y = (uint32_t*)c->scratch.buf.p;
-    }
+    Lease y(need_y ? &c->scratch : nullptr, st);
+    if (need_y) CUDA_TRY(y.acquire(N * pitch * sizeof(uint32_t)));
+    Buffers b{x, y.ptr(), c->d_tw, (uint32_t)pitch, (uint32_t)size};
     std::vector<PassParams> plan = (mode == 2) ? plan_encode(b, N) : plan_ntt(b, N, mode == 1);
-    if (int rc = attach_tables(c, (uint32_t)mode << 8 | ilog2(N), plan, st)) return rc;
-    if (int rc = launch_plan(c, plan, st, timer)) return rc;
-    if (need_y) { std::lock_guard<std::mutex> lk(g_mu); CUDA_TRY(c->scratch.release_to(st)); }
-    return 0;
+    if (int rc = attach_tables(c, {mode == 2 ? kEncode : kNtt, mode == 1, 0, 0, 0, (int)ilog2(N)}, plan, st)) return rc;
+    return launch_plan(c, plan, st, timer);
 }
 
 // N data blocks -> M = N / 2^k parity blocks in rows [0, M) of x (rows [M, N) are left undefined).
@@ -221,53 +262,48 @@ int run_aligned_asym(Context* c, uint32_t* x, size_t N, size_t M, size_t size, s
     size_t M0 = N;                                        // what the passes produce; M0 >= M
     const bool native = N > ((size_t)1 << kMaxLogR);
     if (!native) { if (int rc = run_aligned(c, x, N, size, pitch, 2, st)) return rc; }
-    { std::lock_guard<std::mutex> lk(g_mu); CUDA_TRY(c->scratch.acquire(N * pitch * sizeof(uint32_t), st)); }
-    uint32_t* y = (uint32_t*)c->scratch.buf.p;
+    Lease y(&c->scratch, st);
+    CUDA_TRY(y.acquire(N * pitch * sizeof(uint32_t)));
     if (native) {
         M0 = M;
         while (!asym_native(N, M0)) M0 *= 2;              // M0 = max(M, N1)
-        Buffers b{x, y, c->d_tw, (uint32_t)pitch, (uint32_t)size};
+        Buffers b{x, y.ptr(), c->d_tw, (uint32_t)pitch, (uint32_t)size};
         std::vector<PassParams> plan = plan_encode_asym(b, N, M0);
-        if (int rc = attach_tables(c, 0x40000000u | ilog2(N / M0) << 8 | ilog2(N), plan, st)) return rc;
+        if (int rc = attach_tables(c, {kEncodeAsym, 0, 0, 0, (int)ilog2(N / M0), (int)ilog2(N)}, plan, st)) return rc;
         if (int rc = launch_plan(c, plan, st)) return rc;
     }
     if (M0 != M) {                                        // keep every (M0/M)-th parity block: gather through the scratch buffer
-        CUDA_TRY(cudaMemcpy2DAsync(y, pitch * 4, x, (M0 / M) * pitch * 4, size * 4, M, cudaMemcpyDeviceToDevice, st));
-        CUDA_TRY(cudaMemcpy2DAsync(x, pitch * 4, y, pitch * 4, size * 4, M, cudaMemcpyDeviceToDevice, st));
+        CUDA_TRY(cudaMemcpy2DAsync(y.ptr(), pitch * 4, x, (M0 / M) * pitch * 4, size * 4, M, cudaMemcpyDeviceToDevice, st));
+        CUDA_TRY(cudaMemcpy2DAsync(x, pitch * 4, y.ptr(), pitch * 4, size * 4, M, cudaMemcpyDeviceToDevice, st));
     }
-    { std::lock_guard<std::mutex> lk(g_mu); CUDA_TRY(c->scratch.release_to(st)); }
     return 0;
 }
 
 int run_dev(uint32_t* d, size_t N, size_t size, size_t pitch, int mode, void* stream, const char* who, PassTimer* timer = nullptr)
 {
-    Context* c = g_ctx;
-    if (!c) return fail(FASTECC_B200_ENOINIT, "%s: call fastecc_b200_init() first", who);
-    if (!d) return fail(FASTECC_B200_EINVAL, "%s: null device pointer", who);
+    Context* c = ctx(who);
+    if (!c) return FASTECC_B200_ENOINIT;
     if (int rc = check_shape(N, size, mode == 2 ? FASTECC_B200_MAX_LOG_N_ENCODE : FASTECC_B200_MAX_LOG_N, who, mode != 2)) return rc;
-    if (pitch < size || pitch > 0xFFFFFFF0u) return fail(FASTECC_B200_EINVAL, "%s: pitch_words (%zu) must be in [SIZE_words (%zu), 2^32 - 16]", who, pitch, size);
-    if ((unsigned long long)N * ((pitch + 3) / 4) >= (1ull << 32))
-        return fail(FASTECC_B200_EINVAL, "%s: buffer of %zu x %zu words is 64 GiB or more (32-bit chunk indexing)", who, N, pitch);
+    if (int rc = check_rows(d, N, size, pitch, false, who)) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     const bool aligned = (pitch % 4 == 0) && (((uintptr_t)d) % 16 == 0);
     if (aligned) return run_aligned(c, d, N, size, pitch, mode, st, timer);
     // unaligned layout: repack into a padded copy, transform, copy the SIZE data words back
     const size_t ppitch = (size + 3) / 4 * 4;
-    { std::lock_guard<std::mutex> lk(g_mu); CUDA_TRY(c->packed.acquire(N * ppitch * sizeof(uint32_t), st)); }
-    uint32_t* pk = (uint32_t*)c->packed.buf.p;
-    CUDA_TRY(launch_pack(d, pitch, pk, ppitch, N, (uint32_t)size, st)); g_launches++;
-    if (int rc = run_aligned(c, pk, N, size, ppitch, mode, st, timer)) return rc;
-    CUDA_TRY(launch_unpack(pk, ppitch, d, pitch, N, (uint32_t)size, st)); g_launches++;
-    { std::lock_guard<std::mutex> lk(g_mu); CUDA_TRY(c->packed.release_to(st)); }
+    Lease pk(&c->packed, st);
+    CUDA_TRY(pk.acquire(N * ppitch * sizeof(uint32_t)));
+    CUDA_TRY(launch_pack(d, pitch, pk.ptr(), ppitch, N, (uint32_t)size, st)); g_launches++;
+    if (int rc = run_aligned(c, pk.ptr(), N, size, ppitch, mode, st, timer)) return rc;
+    CUDA_TRY(launch_unpack(pk.ptr(), ppitch, d, pitch, N, (uint32_t)size, st)); g_launches++;
     return 0;
 }
 
-int run_host(uint32_t** data, size_t N, size_t size, int mode, const char* who)
+// The host (T**) entry points: the N blocks are staged in a padded device copy, `transform(x, SIZE, pitch)` runs on it in place
+// on the context's stream, and rows [0, rows_back) are copied back.
+template <class Transform>
+int run_host(Context* c, uint32_t** data, size_t N, size_t rows_back, size_t size, const char* who, Transform transform)
 {
-    Context* c = g_ctx;
-    if (!c) return fail(FASTECC_B200_ENOINIT, "%s: call fastecc_b200_init() first", who);
     if (!data) return fail(FASTECC_B200_EINVAL, "%s: null block table", who);
-    if (int rc = check_shape(N, size, mode == 2 ? FASTECC_B200_MAX_LOG_N_ENCODE : FASTECC_B200_MAX_LOG_N, who, mode != 2)) return rc;
     for (size_t i = 0; i < N; i++) if (!data[i]) return fail(FASTECC_B200_EINVAL, "%s: data[%zu] is null", who, i);
     std::lock_guard<std::mutex> host_lock(g_host_mu);
     const size_t pitch = (size + 3) / 4 * 4;
@@ -277,12 +313,11 @@ int run_host(uint32_t** data, size_t N, size_t size, int mode, const char* who)
     bool contiguous = true;
     for (size_t i = 1; i < N; i++) if (data[i] != data[0] + i * size) { contiguous = false; break; }
     if (pitch != size) CUDA_TRY(cudaMemsetAsync(dv, 0, N * pitch * sizeof(uint32_t), st));
-    // Large contiguous arrays: the word columns are independent codewords, so the array is cut into column chunks and
-    // H2D(chunk c+1), the transform of chunk c and D2H(chunk c-1) run concurrently on three streams (PCIe is full duplex).
-    static const size_t chunk_env = getenv("FASTECC_B200_CHUNK_WORDS") ? (size_t)atol(getenv("FASTECC_B200_CHUNK_WORDS")) : 0;
-    size_t cw = chunk_env ? (chunk_env + 15) / 16 * 16 : 128;
-    const bool pipelined = contiguous && pitch == size && size >= 2 * cw && N * size * 4 >= ((size_t)32 << 20);
-    if (pipelined) {
+    // Large contiguous arrays of which every row comes back: the word columns are independent codewords, so the array is cut
+    // into column chunks and H2D(chunk c+1), the transform of chunk c and D2H(chunk c-1) run concurrently on three streams
+    // (PCIe is full duplex).
+    constexpr size_t cw = 128;                            // words per column chunk
+    if (rows_back == N && contiguous && pitch == size && size >= 2 * cw && N * size * 4 >= ((size_t)32 << 20)) {
         pin_caller_array(c, data[0], N * size * sizeof(uint32_t));
         const size_t nchunks = (size + cw - 1) / cw;
         while (c->ev_in.size() < nchunks) { cudaEvent_t e; CUDA_TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming)); c->ev_in.push_back(e); }
@@ -292,7 +327,7 @@ int run_host(uint32_t** data, size_t N, size_t size, int mode, const char* who)
             CUDA_TRY(cudaMemcpy2DAsync(dv + c0, pitch * 4, data[0] + c0, size * 4, w * 4, N, cudaMemcpyHostToDevice, c->h2d));
             CUDA_TRY(cudaEventRecord(c->ev_in[k], c->h2d));
             CUDA_TRY(cudaStreamWaitEvent(st, c->ev_in[k], 0));
-            if (int rc = run_aligned(c, dv + c0, N, w, pitch, mode, st)) return rc;
+            if (int rc = transform(dv + c0, w, pitch)) return rc;
             CUDA_TRY(cudaEventRecord(c->ev_done[k], st));
             CUDA_TRY(cudaStreamWaitEvent(c->d2h, c->ev_done[k], 0));
             CUDA_TRY(cudaMemcpy2DAsync(data[0] + c0, size * 4, dv + c0, pitch * 4, w * 4, N, cudaMemcpyDeviceToHost, c->d2h));
@@ -301,19 +336,46 @@ int run_host(uint32_t** data, size_t N, size_t size, int mode, const char* who)
         CUDA_TRY(cudaStreamSynchronize(st));
         return 0;
     }
-    if (contiguous) {
-        CUDA_TRY(cudaMemcpy2DAsync(dv, pitch * 4, data[0], size * 4, size * 4, N, cudaMemcpyHostToDevice, st));
-    } else {
-        for (size_t i = 0; i < N; i++) CUDA_TRY(cudaMemcpyAsync(dv + i * pitch, data[i], size * 4, cudaMemcpyHostToDevice, st));
-    }
-    if (int rc = run_aligned(c, dv, N, size, pitch, mode, st)) return rc;
-    if (contiguous) {
-        CUDA_TRY(cudaMemcpy2DAsync(data[0], size * 4, dv, pitch * 4, size * 4, N, cudaMemcpyDeviceToHost, st));
-    } else {
-        for (size_t i = 0; i < N; i++) CUDA_TRY(cudaMemcpyAsync(data[i], dv + i * pitch, size * 4, cudaMemcpyDeviceToHost, st));
-    }
+    if (contiguous) CUDA_TRY(cudaMemcpy2DAsync(dv, pitch * 4, data[0], size * 4, size * 4, N, cudaMemcpyHostToDevice, st));
+    else for (size_t i = 0; i < N; i++) CUDA_TRY(cudaMemcpyAsync(dv + i * pitch, data[i], size * 4, cudaMemcpyHostToDevice, st));
+    if (int rc = transform(dv, size, pitch)) return rc;
+    if (contiguous) CUDA_TRY(cudaMemcpy2DAsync(data[0], size * 4, dv, pitch * 4, size * 4, rows_back, cudaMemcpyDeviceToHost, st));
+    else for (size_t i = 0; i < rows_back; i++) CUDA_TRY(cudaMemcpyAsync(data[i], dv + i * pitch, size * 4, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
     return 0;
+}
+
+int run_host_mode(uint32_t** data, size_t N, size_t size, int mode, const char* who)
+{
+    Context* c = ctx(who);
+    if (!c) return FASTECC_B200_ENOINIT;
+    if (int rc = check_shape(N, size, mode == 2 ? FASTECC_B200_MAX_LOG_N_ENCODE : FASTECC_B200_MAX_LOG_N, who, mode != 2)) return rc;
+    return run_host(c, data, N, N, size, who, [&](uint32_t* x, size_t w, size_t pitch) { return run_aligned(c, x, N, w, pitch, mode, c->stream); });
+}
+
+// One pass of a sharded encode / transform (the three fastecc_b200_*_shard_pass* entry points): kShard (exchange by the
+// caller, `peers` unused), kShardP2P or kNttShardP2P (exchange fused into the stores to `peers`).
+int shard_pass(Kind kind, const uint32_t* src, uint32_t* const* peers, size_t N, int n_ranks, int rank, size_t size, size_t pitch,
+               int inverse, int which, void* stream, const char* who)
+{
+    Context* c = ctx(who);
+    if (!c) return FASTECC_B200_ENOINIT;
+    const bool p2p = kind != kShard;
+    const int passes = kind == kNttShardP2P ? 2 : 3;
+    if (!src || (p2p && !peers) || which < 0 || which >= passes || rank < 0 || rank >= n_ranks) return fail(FASTECC_B200_EINVAL, "%s: bad arguments", who);
+    const uint32_t G = (uint32_t)n_ranks;
+    if (!(kind == kShard ? shard_supported(N, G) : kind == kShardP2P ? shard_p2p_supported(N, G) : ntt_shard_p2p_supported(N, G)))
+        return fail(FASTECC_B200_EINVAL, "%s: N=%zu cannot be sharded over %d ranks (fastecc_b200_shard_geometry tells which can)", who, N, n_ranks);
+    if (int rc = check_rows(src, N / G, size, pitch, true, who)) return rc;
+    for (int r = 0; p2p && r < n_ranks; ++r)
+        if (!peers[r] || ((uintptr_t)peers[r]) % 16) return fail(FASTECC_B200_EINVAL, "%s: peer buffer %d missing or misaligned", who, r);
+    cudaStream_t st = (cudaStream_t)stream;
+    Buffers b{const_cast<uint32_t*>(src), nullptr, c->d_tw, (uint32_t)pitch, (uint32_t)size};
+    std::vector<PassParams> plan{kind == kShard ? plan_encode_shard(b, N, G, (uint32_t)rank, which)
+                                 : kind == kShardP2P ? plan_encode_shard_p2p(src, peers, c->d_tw, (uint32_t)pitch, (uint32_t)size, N, G, (uint32_t)rank, which)
+                                 : plan_ntt_shard_p2p(src, peers, c->d_tw, (uint32_t)pitch, (uint32_t)size, N, G, (uint32_t)rank, inverse != 0, which)};
+    if (int rc = attach_tables(c, {kind, inverse != 0, n_ranks, rank, which, (int)ilog2(N)}, plan, st)) return rc;
+    return launch_plan(c, plan, st);
 }
 
 } // namespace
@@ -322,11 +384,6 @@ int run_host(uint32_t** data, size_t N, size_t size, int mode, const char* who)
 namespace fecc {
 const uint4* context_power_table() { return g_ctx ? g_ctx->d_tw : nullptr; }
 int context_num_sms() { return g_ctx ? g_ctx->num_sms : 0; }
-int api_fail(int code, const char* fmt, ...)
-{
-    va_list ap; va_start(ap, fmt); vsnprintf(g_err, sizeof g_err, fmt, ap); va_end(ap);
-    return code;
-}
 }
 
 extern "C" {
@@ -364,7 +421,7 @@ void fastecc_b200_shutdown(void)
     cudaDeviceSynchronize();
     g_ctx->scratch.destroy(); g_ctx->packed.destroy(); g_ctx->mixed.destroy(); g_ctx->staging.release();
     for (auto& r : g_ctx->registered) cudaHostUnregister(r.first);
-    for (auto& kv : g_ctx->tables) for (auto& sl : kv.second.slots) { sl.buf.release(); if (sl.ready) cudaEventDestroy(sl.ready); }
+    for (auto& kv : g_ctx->tables) for (auto& sl : kv.second) { sl.buf.release(); if (sl.ready) cudaEventDestroy(sl.ready); }
     if (g_ctx->d_tw) cudaFree(g_ctx->d_tw);
     if (g_ctx->stream) cudaStreamDestroy(g_ctx->stream);
     if (g_ctx->h2d) cudaStreamDestroy(g_ctx->h2d);
@@ -414,21 +471,21 @@ int fastecc_b200_shard_geometry(size_t N, int n_ranks, size_t* N1, size_t* N2, i
 
 int fastecc_b200_copy2d_async(void* dst, size_t dst_pitch_bytes, const void* src, size_t src_pitch_bytes, size_t width_bytes, size_t rows, int to_device, void* stream)
 {
-    if (!g_ctx) return fail(FASTECC_B200_ENOINIT, "fastecc_b200_copy2d_async: call fastecc_b200_init() first");
+    if (!ctx("fastecc_b200_copy2d_async")) return FASTECC_B200_ENOINIT;
     CUDA_TRY(cudaMemcpy2DAsync(dst, dst_pitch_bytes, src, src_pitch_bytes, width_bytes, rows, to_device ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToHost, (cudaStream_t)stream));
     return 0;
 }
 
 int fastecc_b200_gf_mul_dev(const uint32_t* a, const uint32_t* b, uint32_t* out, size_t n, void* stream)
 {
-    if (!g_ctx) return fail(FASTECC_B200_ENOINIT, "fastecc_b200_gf_mul_dev: call fastecc_b200_init() first");
+    if (!ctx("fastecc_b200_gf_mul_dev")) return FASTECC_B200_ENOINIT;
     if (n && (!a || !b || !out)) return fail(FASTECC_B200_EINVAL, "fastecc_b200_gf_mul_dev: null device pointer");
     CUDA_TRY(launch_gf_mul(a, b, out, n, (cudaStream_t)stream)); g_launches++;
     return 0;
 }
 int fastecc_b200_gf_inv_dev(const uint32_t* a, uint32_t* out, size_t n, void* stream)
 {
-    if (!g_ctx) return fail(FASTECC_B200_ENOINIT, "fastecc_b200_gf_inv_dev: call fastecc_b200_init() first");
+    if (!ctx("fastecc_b200_gf_inv_dev")) return FASTECC_B200_ENOINIT;
     if (n && (!a || !out)) return fail(FASTECC_B200_EINVAL, "fastecc_b200_gf_inv_dev: null device pointer");
     CUDA_TRY(launch_gf_inv(a, out, n, (cudaStream_t)stream)); g_launches++;
     return 0;
@@ -436,16 +493,17 @@ int fastecc_b200_gf_inv_dev(const uint32_t* a, uint32_t* out, size_t n, void* st
 int fastecc_b200_row_scale_dev(uint32_t* d, size_t n_rows, size_t size, size_t pitch, const uint32_t* d_consts, void* stream)
 {
     const char* who = "fastecc_b200_row_scale_dev";
-    if (!g_ctx) return fail(FASTECC_B200_ENOINIT, "%s: call fastecc_b200_init() first", who);
-    if (!d || !d_consts) return fail(FASTECC_B200_EINVAL, "%s: null device pointer", who);
-    if (size == 0 || pitch < size || pitch > 0xFFFFFFF0u || pitch % 4 || ((uintptr_t)d) % 16) return fail(FASTECC_B200_EINVAL, "%s: needs SIZE >= 1, SIZE <= pitch_words <= 2^32 - 16, pitch %% 4 == 0 and a 16-byte aligned buffer (pad words of a row are scaled too)", who);
-    CUDA_TRY(launch_row_scale(d, n_rows, (uint32_t)((size + 3) / 4), (uint32_t)(pitch / 4), d_consts, g_ctx->num_sms, (cudaStream_t)stream)); g_launches++;
+    Context* c = ctx(who);
+    if (!c) return FASTECC_B200_ENOINIT;
+    if (!d_consts) return fail(FASTECC_B200_EINVAL, "%s: null device pointer", who);
+    if (int rc = check_rows(d, 1, size, pitch, true, who)) return rc;      // one row: the kernel's 32-bit chunk index runs within a row
+    CUDA_TRY(launch_row_scale(d, n_rows, (uint32_t)((size + 3) / 4), (uint32_t)(pitch / 4), d_consts, c->num_sms, (cudaStream_t)stream)); g_launches++;
     return 0;
 }
 
 static int recode_args(const void* a, const void* b, size_t n_blocks, size_t W, size_t pitch, const char* who)
 {
-    if (!g_ctx) return fail(FASTECC_B200_ENOINIT, "%s: call fastecc_b200_init() first", who);
+    if (!ctx(who)) return FASTECC_B200_ENOINIT;
     if (!a || !b) return fail(FASTECC_B200_EINVAL, "%s: null device pointer", who);
     if (W == 0 || W > 1024 || W % 4) return fail(FASTECC_B200_EINVAL, "%s: words_per_block=%zu must be a multiple of 4 in [4, 1024] (10-bit positions, GF.md:84)", who, W);
     if (pitch < W + 1 || pitch % 4) return fail(FASTECC_B200_EINVAL, "%s: pitch_words must be >= words_per_block + 1 and a multiple of 4", who);
@@ -469,105 +527,37 @@ int fastecc_b200_gfp_to_bytes_dev(const uint32_t* d_words, void* d_bytes, size_t
 int fastecc_b200_rs_encode_asym_dev(uint32_t* d, size_t N, size_t M, size_t size, size_t pitch, void* stream)
 {
     const char* who = "fastecc_b200_rs_encode_asym_dev";
-    Context* c = g_ctx;
-    if (!c) return fail(FASTECC_B200_ENOINIT, "%s: call fastecc_b200_init() first", who);
-    if (!d) return fail(FASTECC_B200_EINVAL, "%s: null device pointer", who);
-    if (int rc = check_shape(N, size, FASTECC_B200_MAX_LOG_N_ENCODE, who)) return rc;
-    if (!is_pow2(M) || M > N) return fail(FASTECC_B200_EINVAL, "%s: M=%zu must be a power of two in [1, N]", who, M);
-    if (pitch < size || pitch > 0xFFFFFFF0u || pitch % 4 || ((uintptr_t)d) % 16) return fail(FASTECC_B200_EINVAL, "%s: needs SIZE_words <= pitch_words <= 2^32 - 16, pitch %% 4 == 0 and a 16-byte aligned buffer", who);
-    if ((unsigned long long)N * (pitch / 4) >= (1ull << 32)) return fail(FASTECC_B200_EINVAL, "%s: buffer too large (32-bit chunk indexing)", who);
+    Context* c = ctx(who);
+    if (!c) return FASTECC_B200_ENOINIT;
+    if (int rc = check_asym_shape(N, M, size, who)) return rc;
+    if (int rc = check_rows(d, N, size, pitch, true, who)) return rc;
     return run_aligned_asym(c, d, N, M, size, pitch, (cudaStream_t)stream);
 }
 
 int fastecc_b200_rs_encode_asym(uint32_t** data, size_t N, size_t M, size_t size)
 {
     const char* who = "fastecc_b200_rs_encode_asym";
-    Context* c = g_ctx;
-    if (!c) return fail(FASTECC_B200_ENOINIT, "%s: call fastecc_b200_init() first", who);
-    if (!data) return fail(FASTECC_B200_EINVAL, "%s: null block table", who);
-    if (int rc = check_shape(N, size, FASTECC_B200_MAX_LOG_N_ENCODE, who)) return rc;
-    if (!is_pow2(M) || M > N) return fail(FASTECC_B200_EINVAL, "%s: M=%zu must be a power of two in [1, N]", who, M);
-    for (size_t i = 0; i < N; i++) if (!data[i]) return fail(FASTECC_B200_EINVAL, "%s: data[%zu] is null", who, i);
-    std::lock_guard<std::mutex> host_lock(g_host_mu);
-    const size_t pitch = (size + 3) / 4 * 4;
-    CUDA_TRY(c->staging.reserve(N * pitch * sizeof(uint32_t)));
-    uint32_t* dv = (uint32_t*)c->staging.p;
-    cudaStream_t st = c->stream;
-    bool contiguous = true;
-    for (size_t i = 1; i < N; i++) if (data[i] != data[0] + i * size) { contiguous = false; break; }
-    if (pitch != size) CUDA_TRY(cudaMemsetAsync(dv, 0, N * pitch * sizeof(uint32_t), st));
-    if (contiguous) CUDA_TRY(cudaMemcpy2DAsync(dv, pitch * 4, data[0], size * 4, size * 4, N, cudaMemcpyHostToDevice, st));
-    else for (size_t i = 0; i < N; i++) CUDA_TRY(cudaMemcpyAsync(dv + i * pitch, data[i], size * 4, cudaMemcpyHostToDevice, st));
-    if (int rc = run_aligned_asym(c, dv, N, M, size, pitch, st)) return rc;
-    if (contiguous) CUDA_TRY(cudaMemcpy2DAsync(data[0], size * 4, dv, pitch * 4, size * 4, M, cudaMemcpyDeviceToHost, st));
-    else for (size_t i = 0; i < M; i++) CUDA_TRY(cudaMemcpyAsync(data[i], dv + i * pitch, size * 4, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
-    return 0;
+    Context* c = ctx(who);
+    if (!c) return FASTECC_B200_ENOINIT;
+    if (int rc = check_asym_shape(N, M, size, who)) return rc;
+    return run_host(c, data, N, M, size, who, [&](uint32_t* x, size_t w, size_t pitch) { return run_aligned_asym(c, x, N, M, w, pitch, c->stream); });
 }
 
 int fastecc_b200_rs_encode_shard_pass(uint32_t* d_local, size_t N, int n_ranks, int rank, size_t size, size_t pitch, int which, void* stream)
-{
-    const char* who = "fastecc_b200_rs_encode_shard_pass";
-    Context* c = g_ctx;
-    if (!c) return fail(FASTECC_B200_ENOINIT, "%s: call fastecc_b200_init() first", who);
-    if (!d_local || which < 0 || which > 2 || rank < 0 || rank >= n_ranks) return fail(FASTECC_B200_EINVAL, "%s: bad arguments", who);
-    if (!shard_supported(N, (uint32_t)n_ranks)) return fail(FASTECC_B200_EINVAL, "%s: N=%zu cannot be sharded over %d ranks (need a power of two 2^11..2^19 with N2 %% ranks == 0)", who, N, n_ranks);
-    if (size == 0 || pitch < size || pitch > 0xFFFFFFF0u || pitch % 4 || ((uintptr_t)d_local) % 16) return fail(FASTECC_B200_EINVAL, "%s: needs SIZE >= 1, a 16-byte aligned buffer and pitch %% 4 == 0", who);
-    if ((unsigned long long)(N / n_ranks) * (pitch / 4) >= (1ull << 32)) return fail(FASTECC_B200_EINVAL, "%s: local buffer too large", who);
-    cudaStream_t st = (cudaStream_t)stream;
-    Buffers b{d_local, nullptr, c->d_tw, (uint32_t)pitch, (uint32_t)size};
-    PassParams p = plan_encode_shard(b, N, (uint32_t)n_ranks, (uint32_t)rank, which);
-    std::vector<PassParams> one{p};
-    if (int rc = attach_tables(c, 0x80000000u | (uint32_t)n_ranks << 16 | (uint32_t)rank << 8 | ilog2(N), one, st, which, 3)) return rc;
-    CUDA_TRY(launch_pass(one[0], c->num_sms, st)); g_launches++;
-    return 0;
-}
+{ return shard_pass(kShard, d_local, nullptr, N, n_ranks, rank, size, pitch, 0, which, stream, "fastecc_b200_rs_encode_shard_pass"); }
 
 int fastecc_b200_rs_encode_shard_pass_p2p(const uint32_t* d_src, uint32_t* const* d_peers, size_t N, int n_ranks, int rank, size_t size, size_t pitch,
                                           int which, void* stream)
-{
-    const char* who = "fastecc_b200_rs_encode_shard_pass_p2p";
-    Context* c = g_ctx;
-    if (!c) return fail(FASTECC_B200_ENOINIT, "%s: call fastecc_b200_init() first", who);
-    if (!d_src || !d_peers || which < 0 || which > 2 || rank < 0 || rank >= n_ranks) return fail(FASTECC_B200_EINVAL, "%s: bad arguments", who);
-    if (!shard_p2p_supported(N, (uint32_t)n_ranks))
-        return fail(FASTECC_B200_EINVAL, "%s: N=%zu cannot be sharded over %d ranks with fused exchange (need 2^11..2^19, ranks <= 8 and <= both tile heights / 32)", who, N, n_ranks);
-    if (size == 0 || pitch < size || pitch > 0xFFFFFFF0u || pitch % 4 || ((uintptr_t)d_src) % 16) return fail(FASTECC_B200_EINVAL, "%s: needs SIZE >= 1, 16-byte aligned buffers and pitch %% 4 == 0", who);
-    for (int r = 0; r < n_ranks; ++r)
-        if (!d_peers[r] || ((uintptr_t)d_peers[r]) % 16) return fail(FASTECC_B200_EINVAL, "%s: peer buffer %d missing or misaligned", who, r);
-    if ((unsigned long long)(N / n_ranks) * (pitch / 4) >= (1ull << 32)) return fail(FASTECC_B200_EINVAL, "%s: local buffer too large", who);
-    cudaStream_t st = (cudaStream_t)stream;
-    PassParams p = plan_encode_shard_p2p(d_src, d_peers, c->d_tw, (uint32_t)pitch, (uint32_t)size, N, (uint32_t)n_ranks, (uint32_t)rank, which);
-    std::vector<PassParams> one{p};
-    if (int rc = attach_tables(c, 0xA0000000u | (uint32_t)n_ranks << 16 | (uint32_t)rank << 8 | ilog2(N), one, st, which, 3)) return rc;
-    CUDA_TRY(launch_pass(one[0], c->num_sms, st)); g_launches++;
-    return 0;
-}
+{ return shard_pass(kShardP2P, d_src, d_peers, N, n_ranks, rank, size, pitch, 0, which, stream, "fastecc_b200_rs_encode_shard_pass_p2p"); }
 
 int fastecc_b200_ntt_shard_pass_p2p(const uint32_t* d_src, uint32_t* const* d_peers, size_t N, int n_ranks, int rank, size_t size, size_t pitch,
                                     int inverse, int which, void* stream)
-{
-    const char* who = "fastecc_b200_ntt_shard_pass_p2p";
-    Context* c = g_ctx;
-    if (!c) return fail(FASTECC_B200_ENOINIT, "%s: call fastecc_b200_init() first", who);
-    if (!d_src || !d_peers || which < 0 || which > 1 || rank < 0 || rank >= n_ranks) return fail(FASTECC_B200_EINVAL, "%s: bad arguments", who);
-    if (!ntt_shard_p2p_supported(N, (uint32_t)n_ranks))
-        return fail(FASTECC_B200_EINVAL, "%s: N=%zu cannot be sharded over %d ranks (need 2^11..2^20, ranks <= 8, first tile height >= 32 * ranks)", who, N, n_ranks);
-    if (size == 0 || pitch < size || pitch > 0xFFFFFFF0u || pitch % 4 || ((uintptr_t)d_src) % 16) return fail(FASTECC_B200_EINVAL, "%s: needs SIZE >= 1, 16-byte aligned buffers and pitch %% 4 == 0", who);
-    for (int r = 0; r < n_ranks; ++r)
-        if (!d_peers[r] || ((uintptr_t)d_peers[r]) % 16) return fail(FASTECC_B200_EINVAL, "%s: peer buffer %d missing or misaligned", who, r);
-    if ((unsigned long long)(N / n_ranks) * (pitch / 4) >= (1ull << 32)) return fail(FASTECC_B200_EINVAL, "%s: local buffer too large", who);
-    cudaStream_t st = (cudaStream_t)stream;
-    std::vector<PassParams> one{plan_ntt_shard_p2p(d_src, d_peers, c->d_tw, (uint32_t)pitch, (uint32_t)size, N, (uint32_t)n_ranks, (uint32_t)rank, inverse != 0, which)};
-    if (int rc = attach_tables(c, 0xC0000000u | (inverse ? 1u : 0u) << 28 | (uint32_t)n_ranks << 16 | (uint32_t)rank << 8 | ilog2(N), one, st, which, 2)) return rc;
-    CUDA_TRY(launch_pass(one[0], c->num_sms, st)); g_launches++;
-    return 0;
-}
+{ return shard_pass(kNttShardP2P, d_src, d_peers, N, n_ranks, rank, size, pitch, inverse, which, stream, "fastecc_b200_ntt_shard_pass_p2p"); }
 
 int fastecc_b200_shard_barrier(uint32_t* const* d_flag_peers, int n_ranks, int rank, uint32_t epoch, void* stream)
 {
     const char* who = "fastecc_b200_shard_barrier";
-    if (!g_ctx) return fail(FASTECC_B200_ENOINIT, "%s: call fastecc_b200_init() first", who);
+    if (!ctx(who)) return FASTECC_B200_ENOINIT;
     if (!d_flag_peers || n_ranks < 1 || n_ranks > 8 || rank < 0 || rank >= n_ranks) return fail(FASTECC_B200_EINVAL, "%s: bad arguments", who);
     for (int r = 0; r < n_ranks; ++r) if (!d_flag_peers[r]) return fail(FASTECC_B200_EINVAL, "%s: flag array of rank %d missing", who, r);
     CUDA_TRY(launch_shard_barrier(d_flag_peers, (uint32_t)n_ranks, (uint32_t)rank, epoch, (cudaStream_t)stream)); g_launches++;
@@ -603,7 +593,7 @@ int fastecc_b200_ntt_shard_p2p(uint32_t* const* d_x_peers, uint32_t* const* d_y_
 // allocator hands out sub-blocks, which cannot be exported).
 void* fastecc_b200_dev_alloc(size_t bytes)
 {
-    if (!g_ctx) { fail(FASTECC_B200_ENOINIT, "fastecc_b200_dev_alloc: call fastecc_b200_init() first"); return nullptr; }
+    if (!ctx("fastecc_b200_dev_alloc")) return nullptr;
     void* p = nullptr;
     if (cudaMalloc(&p, bytes) != cudaSuccess) { cudaGetLastError(); fail(FASTECC_B200_ENOMEM, "fastecc_b200_dev_alloc: cudaMalloc(%zu) failed", bytes); return nullptr; }
     return p;
@@ -611,7 +601,7 @@ void* fastecc_b200_dev_alloc(size_t bytes)
 void fastecc_b200_dev_free(void* p) { if (p) cudaFree(p); }
 int fastecc_b200_ipc_export(void* d_ptr, void* handle64)
 {
-    if (!g_ctx) return fail(FASTECC_B200_ENOINIT, "fastecc_b200_ipc_export: call fastecc_b200_init() first");
+    if (!ctx("fastecc_b200_ipc_export")) return FASTECC_B200_ENOINIT;
     static_assert(sizeof(cudaIpcMemHandle_t) == 64, "handle size");
     cudaIpcMemHandle_t h;
     CUDA_TRY(cudaIpcGetMemHandle(&h, d_ptr));
@@ -620,7 +610,7 @@ int fastecc_b200_ipc_export(void* d_ptr, void* handle64)
 }
 int fastecc_b200_ipc_open(const void* handle64, void** d_ptr)
 {
-    if (!g_ctx) return fail(FASTECC_B200_ENOINIT, "fastecc_b200_ipc_open: call fastecc_b200_init() first");
+    if (!ctx("fastecc_b200_ipc_open")) return FASTECC_B200_ENOINIT;
     cudaIpcMemHandle_t h; memcpy(&h, handle64, 64);
     CUDA_TRY(cudaIpcOpenMemHandle(d_ptr, h, cudaIpcMemLazyEnablePeerAccess));
     return 0;
@@ -632,15 +622,15 @@ int fastecc_b200_ipc_close(void* d_ptr)
 }
 
 int fastecc_b200_ntt_u32(uint32_t** data, size_t N, size_t size, int inverse)
-{ return run_host(data, N, size, inverse ? 1 : 0, "fastecc_b200_ntt_u32"); }
+{ return run_host_mode(data, N, size, inverse ? 1 : 0, "fastecc_b200_ntt_u32"); }
 
 int fastecc_b200_rs_encode(uint32_t** data, size_t N, size_t size)
-{ return run_host(data, N, size, 2, "fastecc_b200_rs_encode"); }
+{ return run_host_mode(data, N, size, 2, "fastecc_b200_rs_encode"); }
 
 int fastecc_b200_pin_host_buffers(int enable)
 {
     std::lock_guard<std::mutex> lk(g_host_mu);
-    if (!g_ctx) return fail(FASTECC_B200_ENOINIT, "fastecc_b200_pin_host_buffers: call fastecc_b200_init() first");
+    if (!ctx("fastecc_b200_pin_host_buffers")) return FASTECC_B200_ENOINIT;
     g_ctx->pin_caller = enable != 0;
     if (!enable) {                                                          // turning it off also releases what was page-locked so far
         CUDA_TRY(cudaDeviceSynchronize());

@@ -19,7 +19,7 @@
 namespace fecc {
 const uint4* context_power_table();          // api.cu: g^e, e in [0, 2^20), or nullptr before fastecc_b200_init()
 int          context_num_sms();
-int          api_fail(int code, const char* fmt, ...);
+int          fail(int code, const char* fmt, ...);      // api.cu: records the message for fastecc_b200_last_error()
 }
 
 struct fastecc_b200_erasures {
@@ -130,7 +130,7 @@ struct Scratch {                      // frees what a failed / finished pattern 
 };
 inline size_t pad4(size_t n) { return (n + 3) / 4 * 4; }
 
-#define TRY_CUDA(expr) do { cudaError_t e_ = (expr); if (e_ != cudaSuccess) return api_fail(FASTECC_B200_ECUDA, "%s: %s", #expr, cudaGetErrorString(e_)); } while (0)
+#define TRY_CUDA(expr) do { cudaError_t e_ = (expr); if (e_ != cudaSuccess) return fail(FASTECC_B200_ECUDA, "%s: %s", #expr, cudaGetErrorString(e_)); } while (0)
 #define TRY_RC(expr) do { int rc_ = (expr); if (rc_) return rc_; } while (0)
 
 int build_pattern(fastecc_b200_erasures* E, const uint32_t* erased, cudaStream_t st)
@@ -150,14 +150,14 @@ int build_pattern(fastecc_b200_erasures* E, const uint32_t* erased, cudaStream_t
     size_t groups = 1; while (groups * kLeaf < me) groups *= 2;
     size_t d = kLeaf, cnt = groups, pitch = pad4(cnt);
     uint32_t* polys = tmp.words((d + 1) * pitch);
-    if (!polys) return api_fail(FASTECC_B200_ENOMEM, "fastecc_b200_rs_decode_pattern: out of device memory");
+    if (!polys) return fail(FASTECC_B200_ENOMEM, "fastecc_b200_rs_decode_pattern: out of device memory");
     leaves_kernel<<<GRID(groups), 256, 0, st>>>(E->d_idx, me, 20 - log_n2, tw, polys, groups, pitch);
     // product tree: cnt polynomials of degree <= d  ->  cnt/2 of degree <= 2d
     while (cnt > 1) {
         const size_t rows = 4 * d, half = cnt / 2, hp = pad4(half);
         uint32_t* a = tmp.words(rows * pitch);
         uint32_t* b = tmp.words(rows * hp);
-        if (!a || !b) return api_fail(FASTECC_B200_ENOMEM, "fastecc_b200_rs_decode_pattern: out of device memory");
+        if (!a || !b) return fail(FASTECC_B200_ENOMEM, "fastecc_b200_rs_decode_pattern: out of device memory");
         pad_rows_kernel<<<GRID(rows * pitch), 256, 0, st>>>(polys, pitch, d + 1, a, pitch, rows, cnt);
         TRY_RC(fastecc_b200_ntt_u32_dev(a, rows, cnt, pitch, 0, st));
         if (hp != half) TRY_CUDA(cudaMemsetAsync(b, 0, rows * hp * sizeof(uint32_t), st));      // pad columns: transformed along, never used
@@ -168,7 +168,7 @@ int build_pattern(fastecc_b200_erasures* E, const uint32_t* erased, cudaStream_t
     // l(rho^m) and D = NTT(t * l_t): two single-column transforms of order n2 (16-byte rows)
     uint32_t* lv4 = tmp.words(n2 * 4);
     uint32_t* dl4 = tmp.words(n2 * 4);
-    if (!lv4 || !dl4) return api_fail(FASTECC_B200_ENOMEM, "fastecc_b200_rs_decode_pattern: out of device memory");
+    if (!lv4 || !dl4) return fail(FASTECC_B200_ENOMEM, "fastecc_b200_rs_decode_pattern: out of device memory");
     locator_columns_kernel<<<GRID(n2), 256, 0, st>>>(polys, pitch, d + 1 < n2 ? d + 1 : n2, lv4, dl4, n2);
     TRY_RC(fastecc_b200_ntt_u32_dev(lv4, n2, 1, 4, 0, st));
     TRY_RC(fastecc_b200_ntt_u32_dev(dl4, n2, 1, 4, 0, st));
@@ -185,17 +185,17 @@ extern "C" {
 int fastecc_b200_rs_decode_pattern(size_t n_rows, const uint32_t* erased, size_t n_erased, void* stream, fastecc_b200_erasures** out)
 {
     const char* who = "fastecc_b200_rs_decode_pattern";
-    if (!out) return api_fail(FASTECC_B200_EINVAL, "%s: null output", who);
+    if (!out) return fail(FASTECC_B200_EINVAL, "%s: null output", who);
     *out = nullptr;
-    if (!fecc::context_power_table()) return api_fail(FASTECC_B200_ENOINIT, "%s: call fastecc_b200_init() first", who);
+    if (!fecc::context_power_table()) return fail(FASTECC_B200_ENOINIT, "%s: call fastecc_b200_init() first", who);
     if (n_rows < 2 || (n_rows & (n_rows - 1)) || n_rows > ((size_t)1 << FASTECC_B200_MAX_LOG_N))
-        return api_fail(FASTECC_B200_EINVAL, "%s: the code word must have 2N = 2 .. 2^20 rows (a power of two), got %zu", who, n_rows);
-    if (n_erased > n_rows / 2) return api_fail(FASTECC_B200_EINVAL, "%s: at most N = %zu of the 2N rows can be erased, got %zu", who, n_rows / 2, n_erased);
-    if (n_erased && !erased) return api_fail(FASTECC_B200_EINVAL, "%s: null position list", who);
+        return fail(FASTECC_B200_EINVAL, "%s: the code word must have 2N = 2 .. 2^20 rows (a power of two), got %zu", who, n_rows);
+    if (n_erased > n_rows / 2) return fail(FASTECC_B200_EINVAL, "%s: at most N = %zu of the 2N rows can be erased, got %zu", who, n_rows / 2, n_erased);
+    if (n_erased && !erased) return fail(FASTECC_B200_EINVAL, "%s: null position list", who);
     for (size_t i = 0; i < n_erased; ++i)
-        if (erased[i] >= n_rows || (i && erased[i] <= erased[i - 1])) return api_fail(FASTECC_B200_EINVAL, "%s: erased positions must be ascending, distinct and below %zu", who, n_rows);
+        if (erased[i] >= n_rows || (i && erased[i] <= erased[i - 1])) return fail(FASTECC_B200_EINVAL, "%s: erased positions must be ascending, distinct and below %zu", who, n_rows);
     fastecc_b200_erasures* E = new (std::nothrow) fastecc_b200_erasures;
-    if (!E) return api_fail(FASTECC_B200_ENOMEM, "%s: out of host memory", who);
+    if (!E) return fail(FASTECC_B200_ENOMEM, "%s: out of host memory", who);
     E->n2 = n_rows; E->me = n_erased;
     const int rc = build_pattern(E, erased, (cudaStream_t)stream);
     if (rc) { fastecc_b200_rs_decode_free(E); return rc; }
@@ -206,11 +206,11 @@ int fastecc_b200_rs_decode_pattern(size_t n_rows, const uint32_t* erased, size_t
 int fastecc_b200_rs_decode_recover(const fastecc_b200_erasures* E, uint32_t* d_code, size_t size, size_t pitch, uint32_t* d_out, size_t out_pitch, void* stream)
 {
     const char* who = "fastecc_b200_rs_decode_recover";
-    if (!E || !d_code) return api_fail(FASTECC_B200_EINVAL, "%s: null argument", who);
+    if (!E || !d_code) return fail(FASTECC_B200_EINVAL, "%s: null argument", who);
     if (E->me == 0) return 0;
-    if (!d_out) return api_fail(FASTECC_B200_EINVAL, "%s: null output buffer", who);
+    if (!d_out) return fail(FASTECC_B200_EINVAL, "%s: null output buffer", who);
     if (size == 0 || pitch < size || pitch % 4 || out_pitch < size || out_pitch % 4 || ((uintptr_t)d_code) % 16 || ((uintptr_t)d_out) % 16)
-        return api_fail(FASTECC_B200_EINVAL, "%s: needs SIZE >= 1, 16-byte aligned buffers, pitches >= SIZE and multiples of 4 words", who);
+        return fail(FASTECC_B200_EINVAL, "%s: needs SIZE >= 1, 16-byte aligned buffers, pitches >= SIZE and multiples of 4 words", who);
     cudaStream_t st = (cudaStream_t)stream;
     TRY_RC(fastecc_b200_row_scale_dev(d_code, E->n2, size, pitch, E->d_lv, st));            // p(rho^m) = c[m] * l(rho^m): zero on E whatever was there
     TRY_RC(fastecc_b200_ntt_u32_dev(d_code, E->n2, size, pitch, 1, st));                     // 2N * coefficients of p

@@ -164,7 +164,7 @@ def test_large_mixed_orders_round_trip(fecc, N):
 
 def test_dev_calls_on_two_streams_share_scratch_safely(fecc, oracle):
     """Two-pass NTTs (which ping-pong through the context's ONE scratch buffer) and first-use table builds issued back to back
-    on two different streams: the library orders them with events (csrc/api.cu SharedBuf / TableSet), results must be exact."""
+    on two different streams: the library orders them with events (csrc/api.cu Lease / TableSlot), results must be exact."""
     import torch
     N, S = 1 << 13, 256
     a = ol.fill_B(oracle, N, S)
@@ -404,3 +404,154 @@ def test_argument_validation(fecc):
         fecc.rs_encode_dev(t)
     assert e.value.code == -1
     fecc.ntt_dev(t, False)                                      # but a 2^20 NTT is legal
+
+
+def test_device_entry_point_argument_tables(fecc):
+    """One table of argument tuples per device entry point that takes a row buffer: every rule of its validation, broken on
+    its own, must give FASTECC_B200_EINVAL (-1) before anything is launched, and the valid calls must give 0.  Every pointer
+    lies in ONE device allocation that covers rows x pitch of every tuple (the largest, at the 32-bit chunk-count limit, spans
+    2^36 bytes), so a tuple accepted by mistake stays inside it.  Not listed: the shard passes' upper pitch bound (their
+    smallest buffer at that pitch is 64 rows of 16 GiB) and the ENOINIT check (the session is initialised)."""
+    import ctypes
+    import torch
+    L = fecc.lib()
+    torch.cuda.empty_cache()
+    buf = torch.empty((1 << 34) + (1 << 21), dtype=torch.int32, device="cuda")     # 64 GiB + 8 MiB, never initialised
+    B = buf.data_ptr()
+    C = B + (1 << 36)                                                              # row constants of row_scale: past every row
+    D = B + (1 << 30)                                                              # byte blocks of bytes_to_gfp
+    X0, X1, Y0, Y1 = (B + k * (64 << 20) for k in range(4))                        # the shard passes' X and Y of ranks 0 and 1
+    st = torch.cuda.current_stream().cuda_stream
+    MAXP, BIG = 0xFFFFFFF0, 0xFFFFFFF4                                             # largest pitch / a pitch beyond it
+
+    def peers(*p):
+        return (ctypes.c_void_p * len(p))(*p)
+
+    bad, good = "bad", "good"
+    tables = {
+        "ntt_u32_dev": (L.fastecc_b200_ntt_u32_dev, [        # (d, N, SIZE, pitch, inverse)
+            (bad, 0, 16, 4, 4, 0), (bad, B, 16, 0, 4, 0),
+            (bad, B, 0, 4, 4, 0), (bad, B, 5, 4, 4, 0), (bad, B, 27, 4, 4, 0), (bad, B, 1 << 21, 4, 4, 0), (bad, B, 3 << 21, 4, 4, 0),
+            (bad, B, 1, MAXP + 1, BIG, 0), (bad, B, 3, MAXP + 1, BIG, 1),
+            (bad, B, 16, 8, 4, 0), (bad, B, 1, 4, BIG, 0), (bad, B, 1, 4, MAXP + 1, 0),
+            (bad, B, 1 << 20, 4, 1 << 14, 0), (bad, B, 1 << 20, 4, (1 << 14) - 3, 0),      # 2^20 x ceil(pitch / 4) = 2^32 chunks
+            (good, B, 1 << 12, 64, 64, 0), (good, B, 1 << 12, 64, 64, 1), (good, B, 1 << 20, 4, 4, 0), (good, B, 48, 4, 4, 1),
+            (good, B, 16, 5, 7, 0), (good, B + 4, 16, 4, 4, 0),                       # unaligned layouts are repacked
+        ]),
+        "rs_encode_dev": (L.fastecc_b200_rs_encode_dev, [    # (d, N, SIZE, pitch)
+            (bad, 0, 16, 4, 4), (bad, B, 16, 0, 4),
+            (bad, B, 0, 4, 4), (bad, B, 5, 4, 4), (bad, B, 3, 4, 4), (bad, B, 48, 4, 4), (bad, B, 1 << 20, 4, 4),
+            (bad, B, 1, MAXP + 1, BIG), (bad, B, 16, 8, 4), (bad, B, 1, 4, BIG), (bad, B, 1, 4, MAXP + 1),
+            (bad, B, 1 << 19, 4, 1 << 15), (bad, B, 1 << 19, 4, (1 << 15) - 3),
+            (good, B, 1 << 12, 64, 64), (good, B, 1 << 19, 4, 4), (good, B, 16, 5, 7), (good, B + 4, 16, 4, 4),
+        ]),
+        "rs_encode_asym_dev": (L.fastecc_b200_rs_encode_asym_dev, [      # (d, N, M, SIZE, pitch)
+            (bad, 0, 16, 4, 4, 4), (bad, B, 16, 4, 0, 4),
+            (bad, B, 5, 1, 4, 4), (bad, B, 3, 1, 4, 4), (bad, B, 1 << 20, 1, 4, 4), (bad, B, 1, 1, MAXP + 1, BIG),
+            (bad, B, 16, 0, 4, 4), (bad, B, 16, 3, 4, 4), (bad, B, 16, 32, 4, 4),
+            (bad, B, 16, 4, 8, 4), (bad, B, 1, 1, 4, BIG), (bad, B, 16, 4, 4, 6), (bad, B + 4, 16, 4, 4, 4),
+            (bad, B, 1 << 19, 1, 4, 1 << 15),
+            (good, B, 1 << 12, 1 << 10, 64, 64), (good, B, 16, 4, 4, 4), (good, B, 1 << 19, 1 << 18, 4, 4),
+        ]),
+        "row_scale_dev": (L.fastecc_b200_row_scale_dev, [    # (d, rows, SIZE, pitch, consts)
+            (bad, 0, 16, 4, 4, C), (bad, B, 16, 4, 4, 0), (bad, B, 16, 0, 4, C),
+            (bad, B, 16, 8, 4, C), (bad, B, 1, 4, BIG, C), (bad, B, 16, 4, 6, C), (bad, B + 4, 16, 4, 4, C),
+            (good, B, 77, 36, 40, C), (good, B, 1 << 20, 4, 1 << 14, C),             # no chunk-count limit here
+        ]),
+        "bytes_to_gfp_dev": (L.fastecc_b200_bytes_to_gfp_dev, [          # (bytes, words, n_blocks, W, pitch)
+            (bad, 0, B, 64, 16, 20), (bad, D, 0, 64, 16, 20),
+            (bad, D, B, 64, 0, 4), (bad, D, B, 64, 1028, 1032), (bad, D, B, 64, 6, 8),
+            (bad, D, B, 64, 16, 16), (bad, D, B, 64, 16, 18), (bad, D + 4, B, 64, 16, 20), (bad, D, B + 4, 64, 16, 20),
+            (bad, B, B, 1 << 31, 4, 8),
+            (good, D, B, 64, 16, 20),
+        ]),
+        "rs_encode_shard_pass": (L.fastecc_b200_rs_encode_shard_pass, [  # (d, N, ranks, rank, SIZE, pitch, which)
+            (bad, 0, 1 << 12, 2, 0, 4, 4, 0), (bad, B, 1 << 12, 2, 0, 4, 4, -1), (bad, B, 1 << 12, 2, 0, 4, 4, 3),
+            (bad, B, 1 << 12, 2, -1, 4, 4, 0), (bad, B, 1 << 12, 2, 2, 4, 4, 0), (bad, B, 1 << 12, 0, 0, 4, 4, 0),
+            (bad, B, 1 << 12, 1, 0, 4, 4, 0), (bad, B, 1 << 12, 3, 0, 4, 4, 0), (bad, B, 1 << 10, 2, 0, 4, 4, 0),
+            (bad, B, 1 << 20, 2, 0, 4, 4, 0), (bad, B, 3 << 11, 2, 0, 4, 4, 0), (bad, B, 1 << 11, 64, 0, 4, 4, 0),
+            (bad, B, 1 << 12, 2, 0, 0, 4, 0), (bad, B, 1 << 12, 2, 0, 8, 4, 0), (bad, B, 1 << 12, 2, 0, 4, 6, 0),
+            (bad, B + 4, 1 << 12, 2, 0, 4, 4, 0), (bad, B, 1 << 19, 2, 0, 4, 1 << 16, 0),
+            *[(good, B, 1 << 12, 2, r, 4, 4, w) for r in (0, 1) for w in (0, 1, 2)], (good, B, 1 << 11, 2, 0, 4, 4, 0),
+        ]),
+        "rs_encode_shard_pass_p2p": (L.fastecc_b200_rs_encode_shard_pass_p2p, [      # (src, peers, N, ranks, rank, SIZE, pitch, which)
+            (bad, 0, peers(Y0, Y1), 1 << 12, 2, 0, 4, 4, 0), (bad, X0, None, 1 << 12, 2, 0, 4, 4, 0),
+            (bad, X0, peers(Y0, 0), 1 << 12, 2, 0, 4, 4, 0), (bad, X0, peers(Y0, Y1 + 4), 1 << 12, 2, 0, 4, 4, 0),
+            (bad, X0, peers(Y0 + 4, Y1), 1 << 12, 2, 0, 4, 4, 0),
+            (bad, X0, peers(Y0, Y1), 1 << 12, 2, 0, 4, 4, -1), (bad, X0, peers(Y0, Y1), 1 << 12, 2, 0, 4, 4, 3),
+            (bad, X0, peers(Y0, Y1), 1 << 12, 2, -1, 4, 4, 0), (bad, X0, peers(Y0, Y1), 1 << 12, 2, 2, 4, 4, 0),
+            (bad, X0, peers(Y0), 1 << 12, 1, 0, 4, 4, 0), (bad, X0, peers(Y0, Y1, Y1), 1 << 12, 3, 0, 4, 4, 0),
+            (bad, X0, peers(Y0, Y1), 1 << 11, 2, 0, 4, 4, 0), (bad, X0, peers(Y0, Y1), 1 << 20, 2, 0, 4, 4, 0),
+            (bad, X0, peers(*[Y0] * 16), 1 << 19, 16, 0, 4, 4, 0),
+            (bad, X0, peers(Y0, Y1), 1 << 12, 2, 0, 0, 4, 0), (bad, X0, peers(Y0, Y1), 1 << 12, 2, 0, 8, 4, 0),
+            (bad, X0, peers(Y0, Y1), 1 << 12, 2, 0, 4, 6, 0), (bad, X0 + 4, peers(Y0, Y1), 1 << 12, 2, 0, 4, 4, 0),
+            (bad, B, peers(B, B), 1 << 19, 2, 0, 4, 1 << 16, 0),
+            *[c for r, (x, y) in enumerate(((X0, Y0), (X1, Y1))) for c in (
+                (good, x, peers(Y0, Y1), 1 << 12, 2, r, 4, 4, 0), (good, y, peers(X0, X1), 1 << 12, 2, r, 4, 4, 1),
+                (good, x, peers(X0, X1), 1 << 12, 2, r, 4, 4, 2))],
+        ]),
+        "ntt_shard_pass_p2p": (L.fastecc_b200_ntt_shard_pass_p2p, [      # (src, peers, N, ranks, rank, SIZE, pitch, inverse, which)
+            (bad, 0, peers(Y0, Y1), 1 << 12, 2, 0, 4, 4, 0, 0), (bad, X0, None, 1 << 12, 2, 0, 4, 4, 0, 0),
+            (bad, X0, peers(Y0, 0), 1 << 12, 2, 0, 4, 4, 0, 0), (bad, X0, peers(Y0, Y1 + 4), 1 << 12, 2, 0, 4, 4, 0, 0),
+            (bad, X0, peers(Y0 + 4, Y1), 1 << 12, 2, 0, 4, 4, 0, 0),
+            (bad, X0, peers(Y0, Y1), 1 << 12, 2, 0, 4, 4, 0, -1), (bad, X0, peers(Y0, Y1), 1 << 12, 2, 0, 4, 4, 0, 2),
+            (bad, X0, peers(Y0, Y1), 1 << 12, 2, -1, 4, 4, 0, 0), (bad, X0, peers(Y0, Y1), 1 << 12, 2, 2, 4, 4, 0, 0),
+            (bad, X0, peers(Y0), 1 << 12, 1, 0, 4, 4, 0, 0), (bad, X0, peers(Y0, Y1, Y1), 1 << 12, 3, 0, 4, 4, 0, 0),
+            (bad, X0, peers(Y0, Y1), 1 << 10, 2, 0, 4, 4, 0, 0), (bad, X0, peers(Y0, Y1), 1 << 21, 2, 0, 4, 4, 0, 0),
+            (bad, X0, peers(*[Y0] * 16), 1 << 20, 16, 0, 4, 4, 0, 0),
+            (bad, X0, peers(Y0, Y1), 1 << 12, 2, 0, 0, 4, 0, 0), (bad, X0, peers(Y0, Y1), 1 << 12, 2, 0, 8, 4, 0, 0),
+            (bad, X0, peers(Y0, Y1), 1 << 12, 2, 0, 4, 6, 0, 0), (bad, X0 + 4, peers(Y0, Y1), 1 << 12, 2, 0, 4, 4, 0, 0),
+            (bad, B, peers(B, B), 1 << 20, 2, 0, 4, 1 << 15, 0, 0),
+            *[c for r, (x, y) in enumerate(((X0, Y0), (X1, Y1))) for n in (1 << 11, 1 << 12, 1 << 20) for c in (
+                (good, x, peers(Y0, Y1), n, 2, r, 4, 4, r, 0), (good, y, peers(X0, X1), n, 2, r, 4, 4, r, 1))],
+        ]),
+    }
+    wrong = []
+    for name, (fn, cases) in tables.items():
+        for kind, *args in cases:
+            rc = fn(*args, st)
+            if rc != (0 if kind == good else -1):
+                wrong.append((name, args, rc, L.fastecc_b200_last_error().decode()))
+    torch.cuda.synchronize()
+    del buf
+    torch.cuda.empty_cache()
+    assert not wrong, wrong
+
+
+def test_dev_calls_from_two_host_threads(fecc, oracle):
+    """Two host threads, each on its own stream, run NTTs and encodes of two different two-pass orders (2^12 x 64 and
+    2^15 x 256 words) at the same time; the NTTs of both need the context's one Y buffer, which the larger may have to grow
+    while the other is using it.  Scratch leases (csrc/api.cu) serialise them on the buffer: every result must equal the
+    single-threaded result of the same input, computed afterwards so that the threads meet a buffer that has not grown yet."""
+    import threading
+    import torch
+    inputs = [to_dev(ol.fill_B(oracle, N, S)) for N, S in ((1 << 12, 64), (1 << 15, 256))]
+    ops = [lambda t: fecc.ntt_dev(t, False), lambda t: fecc.ntt_dev(t, True), fecc.rs_encode_dev]
+    torch.cuda.synchronize()
+    results, errors = [[], []], []
+
+    def worker(k):
+        try:
+            s = torch.cuda.Stream()
+            with torch.cuda.stream(s):
+                for i in range(10):
+                    t = inputs[k].clone()
+                    ops[i % len(ops)](t)
+                    results[k].append(t)
+            s.synchronize()
+        except Exception as e:                       # re-raised on the main thread
+            errors.append(e)
+
+    threads = [threading.Thread(target=worker, args=(k,)) for k in range(2)]
+    for th in threads:
+        th.start()
+    for th in threads:
+        th.join()
+    assert not errors, errors
+    for k, x in enumerate(inputs):
+        want = []
+        for op in ops:
+            t = x.clone(); op(t); want.append(t)
+        torch.cuda.synchronize()
+        for i, t in enumerate(results[k]):
+            assert torch.equal(t, want[i % len(ops)]), (k, i)
