@@ -55,6 +55,8 @@ def lib() -> ctypes.CDLL:
         L.fastecc_b200_rs_encode_asym_dev.argtypes = [vp, sz, sz, sz, sz, vp]; L.fastecc_b200_rs_encode_asym_dev.restype = ci
         L.fastecc_b200_rs_encode_mixed.argtypes = [vp, sz, sz]; L.fastecc_b200_rs_encode_mixed.restype = ci
         L.fastecc_b200_rs_encode_mixed_dev.argtypes = [vp, sz, sz, sz, vp]; L.fastecc_b200_rs_encode_mixed_dev.restype = ci
+        L.fastecc_b200_rs_encode_asym_mixed.argtypes = [vp, sz, sz, sz]; L.fastecc_b200_rs_encode_asym_mixed.restype = ci
+        L.fastecc_b200_rs_encode_asym_mixed_dev.argtypes = [vp, sz, sz, sz, sz, vp]; L.fastecc_b200_rs_encode_asym_mixed_dev.restype = ci
         L.fastecc_b200_bytes_to_gfp_dev.argtypes = [vp, vp, sz, sz, sz, vp]; L.fastecc_b200_bytes_to_gfp_dev.restype = ci
         L.fastecc_b200_gfp_to_bytes_dev.argtypes = [vp, vp, sz, sz, sz, vp]; L.fastecc_b200_gfp_to_bytes_dev.restype = ci
         L.fastecc_b200_gf_mul_dev.argtypes = [vp, vp, vp, sz, vp]; L.fastecc_b200_gf_mul_dev.restype = ci
@@ -185,6 +187,14 @@ def EncodeReedSolomon_mixed(data: Blocks, N: int, SIZE: int) -> None:
     del keep
 
 
+def EncodeReedSolomon_asym_mixed(data: Blocks, N: int, M: int, SIZE: int) -> None:
+    """N data blocks (as EncodeReedSolomon_mixed takes them) -> M parity blocks in data[0..M), M any divisor of N: parity
+    block j' = block (N/M)*j' of EncodeReedSolomon_mixed.  Blocks M .. N-1 are left untouched."""
+    tab, keep = _pointer_table(data, N, SIZE)
+    _check(lib().fastecc_b200_rs_encode_asym_mixed(tab.ctypes.data, N, M, SIZE))
+    del keep
+
+
 def rs_code_order(K: int) -> int:
     """The smallest N >= K that EncodeReedSolomon_mixed / rs_encode_mixed_dev accept (2^k, 3 * 2^k or 9 * 2^k, 2^k <= 2^19):
     the number of data blocks to pad K blocks to instead of the next power of two (at most 4/3 K up to K = 2^19, at most 2 K
@@ -239,6 +249,13 @@ def rs_encode_asym_dev(t, M: int) -> None:
     """Rows [0, M) of t receive the M parity blocks; the other rows are undefined afterwards."""
     ptr, N, size, pitch, stream = _dev_args(t)
     _check(lib().fastecc_b200_rs_encode_asym_dev(ptr, N, M, size, pitch, stream))
+
+
+def rs_encode_asym_mixed_dev(t, M: int) -> None:
+    """EncodeReedSolomon_asym_mixed on the rows of a device tensor: rows [0, M) of t receive the M parity blocks (M divides
+    N = t.shape[0]); the other rows are undefined afterwards."""
+    ptr, N, size, pitch, stream = _dev_args(t)
+    _check(lib().fastecc_b200_rs_encode_asym_mixed_dev(ptr, N, M, size, pitch, stream))
 
 
 def bytes_to_gfp_dev(raw, words=None):

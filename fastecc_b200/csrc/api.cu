@@ -146,6 +146,15 @@ int check_asym_shape(size_t N, size_t M, size_t size, const char* who)
     if (!is_pow2(M) || M > N) return fail(FASTECC_B200_EINVAL, "%s: M=%zu must be a power of two in [1, N]", who, M);
     return 0;
 }
+// fastecc_b200_rs_encode_asym_mixed*: N as fastecc_b200_rs_encode_mixed* takes it, M any divisor of N; `pitch` is the row pitch
+// the transforms will run at (the caller's, or the repacked one), of which the order-2^k steps use r times as much
+int check_asym_mixed_shape(size_t N, size_t M, size_t size, size_t pitch, const char* who)
+{
+    if (int rc = check_shape(N, size, FASTECC_B200_MAX_LOG_N_ENCODE, who, true)) return rc;
+    if (M == 0 || M > N || N % M) return fail(FASTECC_B200_EINVAL, "%s: M=%zu must divide N=%zu", who, M, N);
+    if ((unsigned long long)odd_factor(N) * pitch > kMaxPitch) return fail(FASTECC_B200_EINVAL, "%s: %u * pitch_words (%zu) must be <= 2^32 - 16", who, odd_factor(N), pitch);
+    return 0;
+}
 // A device buffer of `rows` rows of `pitch` words, the first SIZE of each meaningful: d != null, 1 <= SIZE <= pitch <= 2^32 - 16,
 // fewer than 2^32 16-byte chunks (the kernels index them in 32 bits); `aligned`: pitch % 4 == 0 and d 16-byte aligned as well.
 int check_rows(const void* d, size_t rows, size_t size, size_t pitch, bool aligned, const char* who)
@@ -289,6 +298,57 @@ int run_aligned_asym(Context* c, uint32_t* x, size_t N, size_t M, size_t size, s
     return 0;
 }
 
+// N = 2^k, 3 * 2^k or 9 * 2^k data blocks -> M parity blocks (M | N) in rows [0, M) of x, rows [M, N) left undefined (DESIGN 3f).
+// N = r * L, D = N / M = s * 2^i: step 1 as in the full encode, step 2 (launch_radix_fold) in place, then the r / s forward
+// transforms of order T = L / 2^f on rows d + r*t, and every 2^(i-f)-th of their outputs gathered into rows [0, M).
+int run_aligned_asym_mixed(Context* c, uint32_t* x, size_t N, size_t M, size_t size, size_t pitch, cudaStream_t st)
+{
+    if (is_pow2(N)) return run_aligned_asym(c, x, N, M, size, pitch, st);
+    if (M == N) return run_aligned(c, x, N, size, pitch, 3, st);
+    const uint32_t r = odd_factor(N), s = odd_factor(N / M), u = r / s;
+    const uint32_t pitch4 = (uint32_t)(pitch / 4), s4 = (uint32_t)((size + 3) / 4);
+    const size_t L = N / r, d2 = N / M / s;
+    const uint32_t log_d2 = ilog2(d2);
+    uint32_t log_fold = 0;                                // fold as far as L / 2^f rows still give every SM 1024 threads
+    while (log_fold < log_d2 && (L >> (log_fold + 1)) * s4 >= (size_t)c->num_sms * 1024) ++log_fold;
+    const size_t T = L >> log_fold, keep = d2 >> log_fold;
+    if (L > 1)                                            // step 1: r inverse transforms of order L, each on every r-th row
+        for (uint32_t n1 = 0; n1 < r; ++n1)
+            if (int rc = run_aligned(c, x + (size_t)n1 * pitch, L, size, (size_t)r * pitch, 1, st)) return rc;
+    CUDA_TRY(launch_radix_fold(x, pitch4, s4, r, (uint32_t)L, s, log_d2, log_fold, c->d_tw, c->num_sms, st)); g_launches++;
+    if (T > 1)                                            // step 3: u forward transforms of order T; parity d + u*j'' lands in row d + r*keep*j''
+        for (uint32_t d = 0; d < u; ++d)
+            if (int rc = run_aligned(c, x + (size_t)d * pitch, T, size, (size_t)r * pitch, 0, st)) return rc;
+    if (u == r && keep == 1) return 0;                    // already rows [0, M)
+    Lease y(&c->scratch, st);                             // gather the groups of u rows through the scratch buffer
+    CUDA_TRY(y.acquire(M * pitch * sizeof(uint32_t)));
+    const size_t groups = M / u, spitch = (size_t)r * keep * pitch * 4, width = ((u - 1) * pitch + size) * 4;
+    if (spitch < ((size_t)1 << 30))
+        CUDA_TRY(cudaMemcpy2DAsync(y.ptr(), u * pitch * 4, x, spitch, width, groups, cudaMemcpyDeviceToDevice, st));
+    else                                                  // beyond what a 2D copy's pitch may be: fewer than 64 groups then (check_rows)
+        for (size_t g = 0; g < groups; ++g)
+            CUDA_TRY(cudaMemcpyAsync(y.ptr() + g * u * pitch, x + g * r * keep * pitch, width, cudaMemcpyDeviceToDevice, st));
+    CUDA_TRY(cudaMemcpy2DAsync(x, pitch * 4, y.ptr(), pitch * 4, size * 4, M, cudaMemcpyDeviceToDevice, st));
+    return 0;
+}
+
+// A device entry point's buffer: run `transform(x, pitch)` on it in place if it is aligned, else on a packed copy of which
+// rows [0, rows_back) are copied back.
+template <class Transform>
+int run_repacked(Context* c, uint32_t* d, size_t N, size_t rows_back, size_t size, size_t pitch, cudaStream_t st, Transform transform)
+{
+    const bool aligned = (pitch % 4 == 0) && (((uintptr_t)d) % 16 == 0);
+    if (aligned) return transform(d, pitch);
+    // unaligned layout: repack into a padded copy, transform, copy the SIZE data words back
+    const size_t ppitch = (size + 3) / 4 * 4;
+    Lease pk(&c->packed, st);
+    CUDA_TRY(pk.acquire(N * ppitch * sizeof(uint32_t)));
+    CUDA_TRY(launch_pack(d, pitch, pk.ptr(), ppitch, N, (uint32_t)size, st)); g_launches++;
+    if (int rc = transform(pk.ptr(), ppitch)) return rc;
+    CUDA_TRY(launch_unpack(pk.ptr(), ppitch, d, pitch, rows_back, (uint32_t)size, st)); g_launches++;
+    return 0;
+}
+
 int run_dev(uint32_t* d, size_t N, size_t size, size_t pitch, int mode, void* stream, const char* who, PassTimer* timer = nullptr)
 {
     Context* c = ctx(who);
@@ -296,16 +356,7 @@ int run_dev(uint32_t* d, size_t N, size_t size, size_t pitch, int mode, void* st
     if (int rc = check_shape(N, size, mode >= 2 ? FASTECC_B200_MAX_LOG_N_ENCODE : FASTECC_B200_MAX_LOG_N, who, mode != 2)) return rc;
     if (int rc = check_rows(d, N, size, pitch, false, who)) return rc;
     cudaStream_t st = (cudaStream_t)stream;
-    const bool aligned = (pitch % 4 == 0) && (((uintptr_t)d) % 16 == 0);
-    if (aligned) return run_aligned(c, d, N, size, pitch, mode, st, timer);
-    // unaligned layout: repack into a padded copy, transform, copy the SIZE data words back
-    const size_t ppitch = (size + 3) / 4 * 4;
-    Lease pk(&c->packed, st);
-    CUDA_TRY(pk.acquire(N * ppitch * sizeof(uint32_t)));
-    CUDA_TRY(launch_pack(d, pitch, pk.ptr(), ppitch, N, (uint32_t)size, st)); g_launches++;
-    if (int rc = run_aligned(c, pk.ptr(), N, size, ppitch, mode, st, timer)) return rc;
-    CUDA_TRY(launch_unpack(pk.ptr(), ppitch, d, pitch, N, (uint32_t)size, st)); g_launches++;
-    return 0;
+    return run_repacked(c, d, N, N, size, pitch, st, [&](uint32_t* x, size_t p) { return run_aligned(c, x, N, size, p, mode, st, timer); });
 }
 
 // The host (T**) entry points: the N blocks are staged in a padded device copy, `transform(x, SIZE, pitch)` runs on it in place
@@ -642,6 +693,27 @@ int fastecc_b200_rs_encode_mixed(uint32_t** data, size_t N, size_t size)
 
 int fastecc_b200_rs_encode_mixed_dev(uint32_t* d, size_t N, size_t size, size_t pitch, void* stream)
 { return run_dev(d, N, size, pitch, 3, stream, "fastecc_b200_rs_encode_mixed_dev"); }
+
+int fastecc_b200_rs_encode_asym_mixed_dev(uint32_t* d, size_t N, size_t M, size_t size, size_t pitch, void* stream)
+{
+    const char* who = "fastecc_b200_rs_encode_asym_mixed_dev";
+    Context* c = ctx(who);
+    if (!c) return FASTECC_B200_ENOINIT;
+    if (int rc = check_rows(d, N, size, pitch, false, who)) return rc;
+    const bool aligned = (pitch % 4 == 0) && (((uintptr_t)d) % 16 == 0);
+    if (int rc = check_asym_mixed_shape(N, M, size, aligned ? pitch : (size + 3) / 4 * 4, who)) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    return run_repacked(c, d, N, M, size, pitch, st, [&](uint32_t* x, size_t p) { return run_aligned_asym_mixed(c, x, N, M, size, p, st); });
+}
+
+int fastecc_b200_rs_encode_asym_mixed(uint32_t** data, size_t N, size_t M, size_t size)
+{
+    const char* who = "fastecc_b200_rs_encode_asym_mixed";
+    Context* c = ctx(who);
+    if (!c) return FASTECC_B200_ENOINIT;
+    if (int rc = check_asym_mixed_shape(N, M, size, (size + 3) / 4 * 4, who)) return rc;
+    return run_host(c, data, N, M, size, who, [&](uint32_t* x, size_t w, size_t pitch) { return run_aligned_asym_mixed(c, x, N, M, w, pitch, c->stream); });
+}
 
 int fastecc_b200_pin_host_buffers(int enable)
 {

@@ -201,4 +201,109 @@ cudaError_t launch_radix_encode(uint32_t* x, uint32_t pitch4, uint32_t s4, uint3
     return cudaGetLastError();
 }
 
+// ---- step 2 of the encode of N = r * M data blocks into N / D parity blocks, D = s * 2^i, s | r (DESIGN 3f) ----------------
+// Only parity p = D*j' is wanted.  With p = j1 + r*j2 (step 3's numbering): p = 0 mod s <=> j1 = 0 mod s, so only the outputs
+// j1 = s*u (u < r/s) of the forward codelet are needed; p = 0 mod 2^i <=> j2 = c_j1 := -j1 * r^-1 mod 2^i.  Multiplying v_j1[k2]
+// by GF_Root(M)^(k2*c_j1) = rho^(2r*k2*c_j1) moves that coset of step 3's outputs to the multiples of 2^i, which the sums
+//     w_j1[t] = sum_{q < 2^f} v'_j1[t + T*q],    T = M / 2^f,  f <= i,
+// followed by a T-point forward transform, produce at every 2^(i-f)-th output.  The twist folds into the output twiddle:
+// rho^(2*k2*J_u), J_u = j1 + r*c_j1 = D*d_u, split by the CRT as in radix_encode_kernel.  Thread (t, chunk) reads the rows
+// r*k2 + n1 of every k2 = t + T*q and writes w_j1[t] to row r*t + d_u -- rows that only it reads, so the pass is in place.
+// f < i leaves T*s4 threads instead of (M / 2^i)*s4 when few parity blocks are wanted (the caller picks f).
+struct FoldConsts {
+    EncodeConsts e;
+    uint32_t tr[9], tm[9];     // 2*J_u*a2 mod r and 2*J_u*b2 mod 2M: rho^(2*k2*J_u) = zeta[tr*k2 mod r] * GF_Root(2M)^(tm*k2 mod 2M)
+    uint32_t d[9];             // output row offset d_u = J_u / D
+};
+
+template <int R, int S>
+__global__ void __launch_bounds__(256) radix_fold_kernel(uint4* __restrict__ x, uint32_t pitch4, uint32_t s4, uint32_t M, uint32_t log_m,
+                                                         uint32_t log_t, uint32_t n_fold, uint32_t a2, uint32_t b2, FoldConsts C, const uint4* __restrict__ tw)
+{
+    constexpr int U = R / S;
+    const size_t total = (size_t)s4 << log_t;
+    const uint32_t mask = 2 * M - 1, sh = 19 - log_m;
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+        const uint32_t t = (uint32_t)(i / s4), c = (uint32_t)(i - (size_t)t * s4);
+        uint32_t acc[U][4];
+#pragma unroll
+        for (int u = 0; u < U; ++u) acc[u][0] = acc[u][1] = acc[u][2] = acc[u][3] = 0;
+        for (uint32_t q = 0; q < n_fold; ++q) {
+            const uint32_t k2 = t + (q << log_t), k2r = k2 % R;
+            const uint4* row = x + (size_t)R * k2 * pitch4 + c;
+            uint32_t f[4][R];
+#pragma unroll
+            for (int n1 = 0; n1 < R; ++n1) {                                    // as radix_encode_kernel
+                const uint4 v = row[(size_t)n1 * pitch4];
+                const uint32_t cr = (uint32_t)(((1 - 2 * n1) % R + R) % R);
+                const uint32_t er = (a2 * ((k2r * cr) % R)) % R, em = (b2 * (k2 * (uint32_t)(1 - 2 * n1))) & mask;
+                const uint4 w = tw[(size_t)em << sh];
+                f[0][n1] = mulc(gf::canon(gf::mul(v.x, w.x, w.y, w.z)), C.e.zin[er]);
+                f[1][n1] = mulc(gf::canon(gf::mul(v.y, w.x, w.y, w.z)), C.e.zin[er]);
+                f[2][n1] = mulc(gf::canon(gf::mul(v.z, w.x, w.y, w.z)), C.e.zin[er]);
+                f[3][n1] = mulc(gf::canon(gf::mul(v.w, w.x, w.y, w.z)), C.e.zin[er]);
+            }
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                dft_r<R>(f[j], C.e.inv);
+#pragma unroll
+                for (int k1 = 1; k1 < R; ++k1) f[j][k1] = mulc(f[j][k1], C.e.sigma[k1]);
+                dft_r<R>(f[j], C.e.fwd);                                        // outputs j1 != 0 mod S are dead code
+            }
+#pragma unroll
+            for (int j = 0; j < 4; ++j) acc[0][j] = addm(acc[0][j], f[j][0]);  // u = 0: J = 0, twiddle 1
+#pragma unroll
+            for (int u = 1; u < U; ++u) {
+                const uint32_t er = (C.tr[u] * k2r) % R, em = (C.tm[u] * k2) & mask;
+                const uint4 w = tw[(size_t)em << sh];
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const uint32_t y = gf::canon(gf::mul(f[j][S * u], w.x, w.y, w.z));
+                    acc[u][j] = addm(acc[u][j], er ? mulc(y, C.e.fwd.zeta[er]) : y);
+                }
+            }
+        }
+        uint4* out = x + (size_t)R * t * pitch4 + c;
+#pragma unroll
+        for (int u = 0; u < U; ++u) out[(size_t)C.d[u] * pitch4] = make_uint4(acc[u][0], acc[u][1], acc[u][2], acc[u][3]);
+    }
+}
+
+cudaError_t launch_radix_fold(uint32_t* x, uint32_t pitch4, uint32_t s4, uint32_t r, uint32_t M, uint32_t s, uint32_t log_d2, uint32_t log_fold,
+                              const uint4* tw, int num_sms, cudaStream_t st)
+{
+    if ((r != 3 && r != 9) || !M || (M & (M - 1)) || M > gf::M / 2 || (s != 1 && s != 3 && s != 9) || r % s || (M >> log_d2) == 0 || log_fold > log_d2)
+        return cudaErrorInvalidValue;
+    uint32_t log_m = 0; while ((1u << log_m) < M) ++log_m;
+    FoldConsts C;
+    fill_codelets(C.e.inv, r, true);
+    fill_codelets(C.e.fwd, r, false);
+    const uint32_t zr = gf::powmod(gf::GEN, (gf::P - 1) / r), sigma = gf::powmod(gf::GEN, (gf::P - 1) / (2 * r)), inv_n = gf::inv(r * M);
+    for (uint32_t j = 0; j < 9; ++j) { fill3(C.e.zin[j], gf::mulmod(gf::powmod(zr, j), inv_n)); fill3(C.e.sigma[j], gf::powmod(sigma, j)); }
+    uint32_t a2 = 0;                                                            // a2 = (2M)^-1 mod r, b2 = r^-1 mod 2M
+    for (uint32_t a = 0; a < r; ++a) if (((uint64_t)a * ((2 * M) % r)) % r == 1) { a2 = a; break; }
+    uint64_t b2 = 1; for (uint32_t i = 0; i <= log_m; ++i) b2 = (b2 * (2 - (r * b2) % (2 * M) + 2 * M)) % (2 * M);
+    const uint64_t d2 = 1ull << log_d2, D = s * d2;
+    uint64_t rinv = 1; for (uint32_t i = 0; i < log_d2; ++i) rinv = (rinv * (2 - (r * rinv) % d2 + d2)) % d2;   // r^-1 mod 2^i
+    for (uint32_t u = 0; u < 9; ++u) {
+        C.tr[u] = C.tm[u] = C.d[u] = 0;
+        if (u >= r / s) continue;
+        const uint64_t j1 = (uint64_t)s * u, cj = (d2 - (j1 * rinv) % d2) % d2, J = j1 + r * cj;   // c_j1 = -j1 * r^-1 mod 2^i
+        C.tr[u] = (uint32_t)((2 * J % r) * a2 % r);
+        C.tm[u] = (uint32_t)((2 * J % (2 * M)) * b2 % (2 * M));
+        C.d[u] = (uint32_t)(J / D);
+    }
+    const uint32_t log_t = log_m - log_fold;
+    const size_t total = (size_t)s4 << log_t;
+    const unsigned grid = (unsigned)((total + 255) / 256 < (size_t)num_sms * 16 ? (total + 255) / 256 : (size_t)num_sms * 16);
+    uint4* x4 = reinterpret_cast<uint4*>(x);
+    const uint32_t nf = 1u << log_fold;
+    if      (r == 3 && s == 1) radix_fold_kernel<3, 1><<<grid, 256, 0, st>>>(x4, pitch4, s4, M, log_m, log_t, nf, a2, (uint32_t)b2, C, tw);
+    else if (r == 3)           radix_fold_kernel<3, 3><<<grid, 256, 0, st>>>(x4, pitch4, s4, M, log_m, log_t, nf, a2, (uint32_t)b2, C, tw);
+    else if (s == 1)           radix_fold_kernel<9, 1><<<grid, 256, 0, st>>>(x4, pitch4, s4, M, log_m, log_t, nf, a2, (uint32_t)b2, C, tw);
+    else if (s == 3)           radix_fold_kernel<9, 3><<<grid, 256, 0, st>>>(x4, pitch4, s4, M, log_m, log_t, nf, a2, (uint32_t)b2, C, tw);
+    else                       radix_fold_kernel<9, 9><<<grid, 256, 0, st>>>(x4, pitch4, s4, M, log_m, log_t, nf, a2, (uint32_t)b2, C, tw);
+    return cudaGetLastError();
+}
+
 } // namespace fecc

@@ -162,6 +162,25 @@ class ErasurePattern:
         return rec
 
 
+def asym_erasures(N: int, M: int, lost_data, lost_parity):
+    """Erased rows of the 2N-row code word (row 2i = data block i, row 2j + 1 = parity block j of the full encode) for the
+    M parity blocks of EncodeReedSolomon_asym_mixed / rs_encode_asym_mixed_dev: 2i for every lost data block i,
+    2*(N/M)*j' + 1 for every lost parity block j', and every odd row that was never produced.  Sorted.  Place the parity with
+    code[1::2*(N//M)] = parity[:M] and decode with CErasurePattern(2N, rows, mixed=True).  ValueError when more than M blocks
+    are lost."""
+    N, M = int(N), int(M)
+    if N < 1 or M < 1 or M > N or N % M:
+        raise ValueError("M = %d must divide N = %d" % (M, N))
+    data, par = sorted({int(i) for i in lost_data}), sorted({int(j) for j in lost_parity})
+    if (data and (data[0] < 0 or data[-1] >= N)) or (par and (par[0] < 0 or par[-1] >= M)):
+        raise ValueError("lost data blocks must lie in [0, N), lost parity blocks in [0, M)")
+    if len(data) + len(par) > M:
+        raise ValueError("%d blocks lost; M = %d parity blocks recover at most %d" % (len(data) + len(par), M, M))
+    D, lost = N // M, set(par)
+    rows = [2 * i for i in data] + [2 * j + 1 for j in range(N) if j % D or j // D in lost]
+    return sorted(rows)
+
+
 class CErasurePattern:
     """The same decoder through the C ABI (fastecc_b200_rs_decode_pattern / _recover: csrc/decode.cu): what a C++ host uses.
     Locator, its values and derivative values are built on the device in one call; recover() is asynchronous.

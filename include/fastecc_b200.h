@@ -105,6 +105,16 @@ int fastecc_b200_rs_encode_asym_dev(uint32_t* d_blocks, size_t N, size_t M, size
 int fastecc_b200_rs_encode_mixed    (uint32_t** data, size_t N, size_t SIZE_words);
 int fastecc_b200_rs_encode_mixed_dev(uint32_t* d_blocks, size_t N, size_t SIZE_words, size_t pitch_words, void* stream);
 
+/* ---- fewer parity blocks than data blocks, for the same orders -------------------------------------------------------
+ * N data blocks in (any N that fastecc_b200_rs_encode_mixed accepts), M parity blocks out, for any M that divides N: parity
+ * block j' is parity block (N/M)*j' of fastecc_b200_rs_encode_mixed, i.e. f(rho^(2*(N/M)*j' + 1)), rho = GF_Root(2N) -- the code
+ * word of 2N rows that fastecc_b200_rs_decode_pattern_mixed decodes, with the parity rows that were not produced erased.  On
+ * return data[j'], j' < M, hold the parity; blocks M .. N-1 are undefined (host variant: left untouched).  Power-of-two N runs
+ * fastecc_b200_rs_encode_asym[_dev] and M = N runs fastecc_b200_rs_encode_mixed[_dev], bit for bit.  Device memory, layouts,
+ * repacking and inputs taken mod P as fastecc_b200_rs_encode_mixed[_dev]. */
+int fastecc_b200_rs_encode_asym_mixed    (uint32_t** data, size_t N, size_t M, size_t SIZE_words);
+int fastecc_b200_rs_encode_asym_mixed_dev(uint32_t* d_blocks, size_t N, size_t M, size_t SIZE_words, size_t pitch_words, void* stream);
+
 /* ---- arbitrary bytes <-> words below P (SURVEY 8f rank 3) -----------------------------------------------------------
  * The reference describes, but does not implement, a bit-optimal recoding (GF.md:72-104, README.md:160-163): the top
  * 12 bits of the W words of a block are rewritten from base 4096 to base 4095 (no 0xFFF, hence every word < P) using

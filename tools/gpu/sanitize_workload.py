@@ -28,6 +28,13 @@ for L, S in ((11, 256), (12, 128), (13, 64), (10, 16), (6, 1024)):
         assert np.array_equal(t[:N // 2].cpu().numpy().view(np.uint32), ol.o_encode(o, a)[::2]), ("asym", L, S)
     b = a.copy(); fe.EncodeReedSolomon_body(b, N, S)
     assert np.array_equal(b, ol.o_encode(o, a)), ("host", L, S)
+for N, M, S in ((3 << 12, (3 << 12) // 8, 16), (3 << 11, 1, 1024)):     # the encode into fewer parity blocks (radix_fold_kernel; folded by 2 in the second)
+    a = ol.fill_B(o, N, S)
+    t = torch.from_numpy(a.view(np.int32)).cuda()
+    fe.rs_encode_asym_mixed_dev(t, M)
+    full = torch.from_numpy(a.view(np.int32)).cuda()
+    fe.rs_encode_mixed_dev(full)
+    assert torch.equal(t[:M], full[::N // M]), ("asym mixed", N, M, S)
 raw = torch.randint(0, 256, (64, 4096), dtype=torch.uint8, device="cuda")
 w = fe.bytes_to_gfp_dev(raw)
 assert bool((fe.gfp_to_bytes_dev(w, 1024) == raw).all())

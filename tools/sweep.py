@@ -2,7 +2,8 @@
 """Device-resident timing sweep over the BASELINE parity configs (SURVEY 8d: configs 1, 3 and the NTT sweep 5):
 encode at N = 2^7 .. 2^19 and forward NTT at N = 2^10 .. 2^20, 4096-byte blocks, CUDA events around `reps` back-to-back
 calls.  Arrays below ~100 MB stay in the 126 MB L2 between calls (marked); the small orders are launch-latency bound.
-Then recoding, decoding, the asymmetric encode and the encode of 3 * 2^k / 9 * 2^k blocks (`encode_mixed`, DESIGN 3e).
+Then recoding, decoding, the asymmetric encode, the encode of 3 * 2^k / 9 * 2^k blocks (`encode_mixed`, DESIGN 3e) and
+their encode into fewer parity blocks (`encode_asym_mixed`, DESIGN 3f; `--asym-mixed`: only these).
 Prints one JSON line per point."""
 import json
 import os
@@ -34,6 +35,9 @@ def timed(fn, reps):
 def main():
     fe.init(0)
     S = 1024
+    if "--asym-mixed" in sys.argv:                            # only the encode_asym_mixed lines
+        asym_mixed_encode(S)
+        return 0
     only_extras = "--extras" in sys.argv
     for op, Ls in (() if only_extras else (("encode", range(7, 20)), ("ntt", range(10, 21)))):
         for L in Ls:
@@ -84,6 +88,7 @@ def main():
         del x
         torch.cuda.empty_cache()
     mixed_encode(S)
+    asym_mixed_encode(S)
     return 0
 
 
@@ -141,6 +146,42 @@ def mixed_encode(S):
                           "GBps_kernel_read_plus_write": round(2 * nbytes / (us / n) / 1e3, 1) if n else None,
                           "MiBps_reference_convention": round(2 * nbytes / 2**20 / min(ms_mixed, ms_mixed_again) * 1e3)}), flush=True)
         del x, consts
+        torch.cuda.empty_cache()
+
+
+def asym_mixed_encode(S):
+    """N = 3 * 2^k / 9 * 2^k data blocks into M = N/2, N/r, N/8, N/64 parity blocks (fastecc_b200_rs_encode_asym_mixed_dev,
+    DESIGN 3f) against the full encode of the same array (rs_encode_mixed_dev), timed alternately, twice each; the lower
+    figures.  Every line carries the card's name and power limit, read in the same run."""
+    from bench import gpu_identity
+    card = gpu_identity(torch.cuda.current_device())
+    for N in (3 << 16, 9 << 15, 3 << 17, 9 << 16, 3 << 18, 9 << 17, 3 << 19, 9 << 18):
+        r = 3 if N % 9 else 9
+        x = (torch.arange(N * S, device="cuda", dtype=torch.int64) % P).to(torch.int32).view(N, S)
+        reps = max(5, min(50, int(4e9 // (N * S * 4))))
+        for M in (N // 2, N // r, N // 8, N // 64):
+            runs_asym, runs_full = [], []
+            for _ in range(2):
+                runs_full.append(timed(lambda: fe.rs_encode_mixed_dev(x), reps))
+                runs_asym.append(timed(lambda: fe.rs_encode_asym_mixed_dev(x, M), reps))
+            ms, ms_full = min(runs_asym), min(runs_full)
+            from torch.profiler import ProfilerActivity, profile
+            with profile(activities=[ProfilerActivity.CUDA]) as prof:               # a profiled loop of its own, after the timed ones
+                for _ in range(reps):
+                    fe.rs_encode_asym_mixed_dev(x, M)
+                torch.cuda.synchronize()
+            dev_ms = {}
+            for e in prof.key_averages():
+                us = getattr(e, "device_time_total", 0) or getattr(e, "cuda_time_total", 0)
+                if us:
+                    k = "radix_fold_kernel" if "radix_fold_kernel" in e.key else "memcpy" if "emcpy" in e.key else "transforms"
+                    dev_ms[k] = dev_ms.get(k, 0) + us / 1e3 / reps
+            print(json.dumps({"op": "encode_asym_mixed", "N": N, "M": M, "r": r, "block_bytes": 4 * S, "reps": reps,
+                              "ms": round(ms, 5), "ms_runs": [round(v, 5) for v in runs_asym],
+                              "ms_full_mixed_encode": round(ms_full, 5), "ms_full_runs": [round(v, 5) for v in runs_full],
+                              "ratio": round(ms / ms_full, 3), "profiled_ms": {k: round(v, 4) for k, v in sorted(dev_ms.items())},
+                              "gpu": card["name"], "power_limit_w": card["power_limit_w"]}), flush=True)
+        del x
         torch.cuda.empty_cache()
 
 
