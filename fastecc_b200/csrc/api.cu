@@ -122,39 +122,23 @@ Context* ctx(const char* who)
     return g_ctx;
 }
 
-// N = r * 2^k with r = 3 or 9: the orders served by mixed_radix.cu on top of the power-of-two kernels (transforms, and the
-// encode of fastecc_b200_rs_encode_mixed*)
-uint32_t odd_factor(size_t N)
-{
-    if (!N) return 0;
-    while (!(N & 1)) N >>= 1;
-    return (uint32_t)(N <= 9 ? N : 0);
-}
 constexpr size_t kMaxPitch = 0xFFFFFFF0u;
-int check_shape(size_t N, size_t size, size_t max_log, const char* who, bool allow_mixed = false)
+// The shape of every transform and encode, checked before anything is allocated, copied or launched: SIZE in [1, 2^32 - 16];
+// N = r * 2^k with 2^k <= 2^max_log and r = 1, or r in {3, 9} if `mixed_ok` (mixed_radix.cu); M divides N (the M parity blocks
+// of an encode; M = N for a transform); r * run_pitch <= 2^32 - 16, since the order-2^k steps of r > 1 run on every r-th row of
+// the buffer at the row pitch `run_pitch` (the caller's for an aligned layout, ceil(SIZE / 4) * 4 for a repacked or staged one).
+int check_order(size_t N, size_t M, size_t size, size_t run_pitch, size_t max_log, bool mixed_ok, const char* who)
 {
     if (size == 0 || size > kMaxPitch) return fail(FASTECC_B200_EINVAL, "%s: SIZE_words=%zu must be in [1, 2^32 - 16]", who, size);
-    const uint32_t r = odd_factor(N);
-    const size_t pow2_part = allow_mixed && (r == 3 || r == 9) ? N / r : N;
-    if (!is_pow2(pow2_part) || pow2_part > ((size_t)1 << max_log))
-        return fail(FASTECC_B200_EINVAL, "%s: N=%zu must be a power of two in [1, 2^%zu]%s (P-1 = 2^20*4095)", who, N, max_log, allow_mixed ? ", or 3 or 9 times one" : "");
+    const Order o = split_order(N);
+    if (!o.r || (o.r != 1 && !mixed_ok) || o.log2_m > max_log)
+        return fail(FASTECC_B200_EINVAL, "%s: N=%zu must be a power of two in [1, 2^%zu]%s (P-1 = 2^20*4095)", who, N, max_log, mixed_ok ? ", or 3 or 9 times one" : "");
+    if (M == 0 || N % M) return fail(FASTECC_B200_EINVAL, "%s: M=%zu must divide N=%zu", who, M, N);
+    if ((unsigned long long)o.r * run_pitch > kMaxPitch) return fail(FASTECC_B200_EINVAL, "%s: %u * pitch_words (%zu) must be <= 2^32 - 16", who, o.r, run_pitch);
     return 0;
 }
-int check_asym_shape(size_t N, size_t M, size_t size, const char* who)
-{
-    if (int rc = check_shape(N, size, FASTECC_B200_MAX_LOG_N_ENCODE, who)) return rc;
-    if (!is_pow2(M) || M > N) return fail(FASTECC_B200_EINVAL, "%s: M=%zu must be a power of two in [1, N]", who, M);
-    return 0;
-}
-// fastecc_b200_rs_encode_asym_mixed*: N as fastecc_b200_rs_encode_mixed* takes it, M any divisor of N; `pitch` is the row pitch
-// the transforms will run at (the caller's, or the repacked one), of which the order-2^k steps use r times as much
-int check_asym_mixed_shape(size_t N, size_t M, size_t size, size_t pitch, const char* who)
-{
-    if (int rc = check_shape(N, size, FASTECC_B200_MAX_LOG_N_ENCODE, who, true)) return rc;
-    if (M == 0 || M > N || N % M) return fail(FASTECC_B200_EINVAL, "%s: M=%zu must divide N=%zu", who, M, N);
-    if ((unsigned long long)odd_factor(N) * pitch > kMaxPitch) return fail(FASTECC_B200_EINVAL, "%s: %u * pitch_words (%zu) must be <= 2^32 - 16", who, odd_factor(N), pitch);
-    return 0;
-}
+bool is_aligned(const void* d, size_t pitch) { return pitch % 4 == 0 && (uintptr_t)d % 16 == 0; }
+size_t padded_pitch(size_t size) { return (size + 3) / 4 * 4; }
 // A device buffer of `rows` rows of `pitch` words, the first SIZE of each meaningful: d != null, 1 <= SIZE <= pitch <= 2^32 - 16,
 // fewer than 2^32 16-byte chunks (the kernels index them in 32 bits); `aligned`: pitch % 4 == 0 and d 16-byte aligned as well.
 int check_rows(const void* d, size_t rows, size_t size, size_t pitch, bool aligned, const char* who)
@@ -231,94 +215,97 @@ int launch_plan(Context* c, std::vector<PassParams>& plan, cudaStream_t st, Pass
     return 0;
 }
 
-// Run the planned passes on an aligned, padded device buffer.
-// mode 3: the encode of N = 2^k (= mode 2), 3 * 2^k or 9 * 2^k data blocks (fastecc_b200_rs_encode_mixed*).
-int run_aligned(Context* c, uint32_t* x, size_t N, size_t size, size_t pitch, int mode /*0 fwd,1 inv,2 encode,3 encode mixed*/, cudaStream_t st, PassTimer* timer = nullptr)
+// N < 2^kMinLogR: one small-DFT launch, the transform of order N or (`encode`) the whole encode of N data blocks.
+int small_dft(Context* c, uint32_t* x, size_t N, size_t size, size_t pitch, bool inverse, bool encode, cudaStream_t st)
 {
-    const uint32_t pitch4 = (uint32_t)(pitch / 4), s4 = (uint32_t)((size + 3) / 4);
-    if (mode == 3 && is_pow2(N)) mode = 2;
-    if (!is_pow2(N)) {                                    // N = r * M, r = 3 or 9 (mixed_radix.cu)
-        const uint32_t r = odd_factor(N);
-        const size_t M = N / r;
-        if (mode == 2 || (r != 3 && r != 9) || (unsigned long long)r * pitch > 0xFFFFFFF0ull) return fail(FASTECC_B200_EINVAL, "unsupported order N=%zu", N);
-        if (M > 1)                                        // step 1: r transforms of order M, each on every r-th row (row pitch r times larger), in place
-            for (uint32_t n1 = 0; n1 < r; ++n1)
-                if (int rc = run_aligned(c, x + (size_t)n1 * pitch, M, size, (size_t)r * pitch, mode == 3 ? 1 : mode, st)) return rc;
-        if (mode == 3) {                                  // encode (DESIGN 3e): step 2 in place on the r adjacent rows, then r forward transforms
-            CUDA_TRY(launch_radix_encode(x, pitch4, s4, r, (uint32_t)M, c->d_tw, c->num_sms, st)); g_launches++;
-            if (M > 1)
-                for (uint32_t j1 = 0; j1 < r; ++j1)
-                    if (int rc = run_aligned(c, x + (size_t)j1 * pitch, M, size, (size_t)r * pitch, 0, st)) return rc;
-            return 0;
-        }
-        Lease y(&c->mixed, st);                           // step 2: twiddles + order-r transform, into natural order (out of place), then back
-        CUDA_TRY(y.acquire(N * pitch * sizeof(uint32_t)));
-        CUDA_TRY(launch_radix_pass(x, y.ptr(), pitch4, s4, r, (uint32_t)M, mode == 1, c->d_tw, c->num_sms, st)); g_launches++;
-        CUDA_TRY(cudaMemcpy2DAsync(x, pitch * 4, y.ptr(), pitch * 4, (size_t)s4 * 16 < pitch * 4 ? (size_t)s4 * 16 : pitch * 4, N, cudaMemcpyDeviceToDevice, st));
-        return 0;
-    }
-    if (N < ((size_t)1 << kMinLogR)) {
-        const uint32_t z = (uint32_t)(gf::M / N) * (mode == 1 ? (uint32_t)-1 : 1u) & (gf::M - 1);
-        const uint32_t q = mode == 2 ? (uint32_t)(gf::M / (2 * N)) : 0;
-        const gf::Tw in = gf::make_tw(gf::inv((uint32_t)N));
-        CUDA_TRY(launch_small_dft(x, pitch4, s4, (uint32_t)N, z, mode == 2, q, make_uint4(in.w, in.whi, in.wlo, 0), c->d_tw, st));
-        g_launches++;
-        return 0;
-    }
-    const bool need_y = mode != 2 && !single_pass(ilog2(N));               // the two-pass NTT ping-pongs through Y
-    Lease y(need_y ? &c->scratch : nullptr, st);
-    if (need_y) CUDA_TRY(y.acquire(N * pitch * sizeof(uint32_t)));
-    Buffers b{x, y.ptr(), c->d_tw, (uint32_t)pitch, (uint32_t)size};
-    std::vector<PassParams> plan = (mode == 2) ? plan_encode(b, N) : plan_ntt(b, N, mode == 1);
-    if (int rc = attach_tables(c, {mode == 2 ? kEncode : kNtt, mode == 1, 0, 0, 0, (int)ilog2(N)}, plan, st)) return rc;
-    return launch_plan(c, plan, st, timer);
-}
-
-// N data blocks -> M = N / 2^k parity blocks in rows [0, M) of x (rows [M, N) are left undefined).
-int run_aligned_asym(Context* c, uint32_t* x, size_t N, size_t M, size_t size, size_t pitch, cudaStream_t st)
-{
-    if (M == N) return run_aligned(c, x, N, size, pitch, 2, st);
-    size_t M0 = N;                                        // what the passes produce; M0 >= M
-    const bool native = N > ((size_t)1 << kMaxLogR);
-    if (!native) { if (int rc = run_aligned(c, x, N, size, pitch, 2, st)) return rc; }
-    Lease y(&c->scratch, st);
-    CUDA_TRY(y.acquire(N * pitch * sizeof(uint32_t)));
-    if (native) {
-        M0 = M;
-        while (!asym_native(N, M0)) M0 *= 2;              // M0 = max(M, N1)
-        Buffers b{x, y.ptr(), c->d_tw, (uint32_t)pitch, (uint32_t)size};
-        std::vector<PassParams> plan = plan_encode_asym(b, N, M0);
-        if (int rc = attach_tables(c, {kEncodeAsym, 0, 0, 0, (int)ilog2(N / M0), (int)ilog2(N)}, plan, st)) return rc;
-        if (int rc = launch_plan(c, plan, st)) return rc;
-    }
-    if (M0 != M) {                                        // keep every (M0/M)-th parity block: gather through the scratch buffer
-        CUDA_TRY(cudaMemcpy2DAsync(y.ptr(), pitch * 4, x, (M0 / M) * pitch * 4, size * 4, M, cudaMemcpyDeviceToDevice, st));
-        CUDA_TRY(cudaMemcpy2DAsync(x, pitch * 4, y.ptr(), pitch * 4, size * 4, M, cudaMemcpyDeviceToDevice, st));
-    }
+    const uint32_t z = (uint32_t)(gf::M / N) * (inverse ? (uint32_t)-1 : 1u) & (gf::M - 1);
+    const uint32_t q = encode ? (uint32_t)(gf::M / (2 * N)) : 0;
+    const gf::Tw in = gf::make_tw(gf::inv((uint32_t)N));
+    CUDA_TRY(launch_small_dft(x, (uint32_t)(pitch / 4), (uint32_t)((size + 3) / 4), (uint32_t)N, z, encode, q, make_uint4(in.w, in.whi, in.wlo, 0), c->d_tw, st));
+    g_launches++;
     return 0;
 }
 
-// N = 2^k, 3 * 2^k or 9 * 2^k data blocks -> M parity blocks (M | N) in rows [0, M) of x, rows [M, N) left undefined (DESIGN 3f).
-// N = r * L, D = N / M = s * 2^i: step 1 as in the full encode, step 2 (launch_radix_fold) in place, then the r / s forward
-// transforms of order T = L / 2^f on rows d + r*t, and every 2^(i-f)-th of their outputs gathered into rows [0, M).
-int run_aligned_asym_mixed(Context* c, uint32_t* x, size_t N, size_t M, size_t size, size_t pitch, cudaStream_t st)
+// The transform of order N = 2^k, 3 * 2^k or 9 * 2^k, in place on an aligned, padded device buffer.
+int ntt(Context* c, uint32_t* x, size_t N, size_t size, size_t pitch, bool inverse, cudaStream_t st)
 {
-    if (is_pow2(N)) return run_aligned_asym(c, x, N, M, size, pitch, st);
-    if (M == N) return run_aligned(c, x, N, size, pitch, 3, st);
-    const uint32_t r = odd_factor(N), s = odd_factor(N / M), u = r / s;
+    const Order o = split_order(N);
+    if (o.r > 1) {                                        // N = r * L (mixed_radix.cu)
+        const size_t L = N / o.r;
+        if (L > 1)                                        // step 1: r transforms of order L, each on every r-th row (row pitch r times larger), in place
+            for (uint32_t n1 = 0; n1 < o.r; ++n1)
+                if (int rc = ntt(c, x + (size_t)n1 * pitch, L, size, (size_t)o.r * pitch, inverse, st)) return rc;
+        const uint32_t pitch4 = (uint32_t)(pitch / 4), s4 = (uint32_t)((size + 3) / 4);
+        Lease y(&c->mixed, st);                           // step 2: twiddles + order-r transform, into natural order (out of place), then back
+        CUDA_TRY(y.acquire(N * pitch * sizeof(uint32_t)));
+        CUDA_TRY(launch_radix_pass(x, y.ptr(), pitch4, s4, o.r, (uint32_t)L, inverse, c->d_tw, c->num_sms, st)); g_launches++;
+        CUDA_TRY(cudaMemcpy2DAsync(x, pitch * 4, y.ptr(), pitch * 4, (size_t)s4 * 16 < pitch * 4 ? (size_t)s4 * 16 : pitch * 4, N, cudaMemcpyDeviceToDevice, st));
+        return 0;
+    }
+    if (N < ((size_t)1 << kMinLogR)) return small_dft(c, x, N, size, pitch, inverse, false, st);
+    const bool need_y = !single_pass(ilog2(N));                              // the two-pass NTT ping-pongs through Y
+    Lease y(need_y ? &c->scratch : nullptr, st);
+    if (need_y) CUDA_TRY(y.acquire(N * pitch * sizeof(uint32_t)));
+    Buffers b{x, y.ptr(), c->d_tw, (uint32_t)pitch, (uint32_t)size};
+    std::vector<PassParams> plan = plan_ntt(b, N, inverse);
+    if (int rc = attach_tables(c, {kNtt, inverse, 0, 0, 0, (int)ilog2(N)}, plan, st)) return rc;
+    return launch_plan(c, plan, st);
+}
+
+// The whole encode of a power-of-two N: one small-DFT launch or the passes of plan_encode (timed for rs_encode_dev_timed).
+int encode_pow2(Context* c, uint32_t* x, size_t N, size_t size, size_t pitch, cudaStream_t st, PassTimer* timer)
+{
+    if (N < ((size_t)1 << kMinLogR)) return small_dft(c, x, N, size, pitch, false, true, st);
+    Buffers b{x, nullptr, c->d_tw, (uint32_t)pitch, (uint32_t)size};
+    std::vector<PassParams> plan = plan_encode(b, N);
+    if (int rc = attach_tables(c, {kEncode, 0, 0, 0, 0, (int)ilog2(N)}, plan, st)) return rc;
+    return launch_plan(c, plan, st, timer);
+}
+
+// N = 2^k, 3 * 2^k or 9 * 2^k data blocks -> M parity blocks (M | N) in rows [0, M) of an aligned, padded device buffer; rows
+// [M, N) are left undefined.
+int encode(Context* c, uint32_t* x, size_t N, size_t M, size_t size, size_t pitch, cudaStream_t st, PassTimer* timer = nullptr)
+{
+    const Order ord = split_order(N), ratio = split_order(N / M);            // N = r * L, D = N / M = s * 2^i
+    if (ord.r == 1 && M == N) return encode_pow2(c, x, N, size, pitch, st, timer);
+    if (ord.r == 1) {                                     // power of two, M = N / 2^i
+        size_t M0 = N;                                    // what the passes produce; M0 >= M
+        const bool native = N > ((size_t)1 << kMaxLogR);
+        if (!native) { if (int rc = encode_pow2(c, x, N, size, pitch, st, nullptr)) return rc; }
+        Lease y(&c->scratch, st);
+        CUDA_TRY(y.acquire(N * pitch * sizeof(uint32_t)));
+        if (native) {
+            M0 = M;
+            while (!asym_native(N, M0)) M0 *= 2;          // M0 = max(M, N1)
+            Buffers b{x, y.ptr(), c->d_tw, (uint32_t)pitch, (uint32_t)size};
+            std::vector<PassParams> plan = plan_encode_asym(b, N, M0);
+            if (int rc = attach_tables(c, {kEncodeAsym, 0, 0, 0, (int)ilog2(N / M0), (int)ilog2(N)}, plan, st)) return rc;
+            if (int rc = launch_plan(c, plan, st)) return rc;
+        }
+        if (M0 != M) {                                    // keep every (M0/M)-th parity block: gather through the scratch buffer
+            CUDA_TRY(cudaMemcpy2DAsync(y.ptr(), pitch * 4, x, (M0 / M) * pitch * 4, size * 4, M, cudaMemcpyDeviceToDevice, st));
+            CUDA_TRY(cudaMemcpy2DAsync(x, pitch * 4, y.ptr(), pitch * 4, size * 4, M, cudaMemcpyDeviceToDevice, st));
+        }
+        return 0;
+    }
+    // N = r * L (DESIGN 3e, 3f): step 1, r inverse transforms of order L on every r-th row; step 2 in place, launch_radix_encode
+    // for D = 1, else launch_radix_fold; step 3, the r / s forward transforms of order T = L / 2^f on rows d + r*t, of whose
+    // outputs every 2^(i-f)-th is gathered into rows [0, M).
+    const uint32_t r = ord.r, s = ratio.r, u = r / s, log_d2 = ratio.log2_m;
     const uint32_t pitch4 = (uint32_t)(pitch / 4), s4 = (uint32_t)((size + 3) / 4);
-    const size_t L = N / r, d2 = N / M / s;
-    const uint32_t log_d2 = ilog2(d2);
+    const size_t L = N / r;
     uint32_t log_fold = 0;                                // fold as far as L / 2^f rows still give every SM 1024 threads
     while (log_fold < log_d2 && (L >> (log_fold + 1)) * s4 >= (size_t)c->num_sms * 1024) ++log_fold;
-    const size_t T = L >> log_fold, keep = d2 >> log_fold;
-    if (L > 1)                                            // step 1: r inverse transforms of order L, each on every r-th row
+    const size_t T = L >> log_fold, keep = ((size_t)1 << log_d2) >> log_fold;
+    if (L > 1)
         for (uint32_t n1 = 0; n1 < r; ++n1)
-            if (int rc = run_aligned(c, x + (size_t)n1 * pitch, L, size, (size_t)r * pitch, 1, st)) return rc;
-    CUDA_TRY(launch_radix_fold(x, pitch4, s4, r, (uint32_t)L, s, log_d2, log_fold, c->d_tw, c->num_sms, st)); g_launches++;
-    if (T > 1)                                            // step 3: u forward transforms of order T; parity d + u*j'' lands in row d + r*keep*j''
+            if (int rc = ntt(c, x + (size_t)n1 * pitch, L, size, (size_t)r * pitch, true, st)) return rc;
+    if (M == N) CUDA_TRY(launch_radix_encode(x, pitch4, s4, r, (uint32_t)L, c->d_tw, c->num_sms, st));
+    else        CUDA_TRY(launch_radix_fold(x, pitch4, s4, r, (uint32_t)L, s, log_d2, log_fold, c->d_tw, c->num_sms, st));
+    g_launches++;
+    if (T > 1)                                            // parity d + u*j'' lands in row d + r*keep*j''
         for (uint32_t d = 0; d < u; ++d)
-            if (int rc = run_aligned(c, x + (size_t)d * pitch, T, size, (size_t)r * pitch, 0, st)) return rc;
+            if (int rc = ntt(c, x + (size_t)d * pitch, T, size, (size_t)r * pitch, false, st)) return rc;
     if (u == r && keep == 1) return 0;                    // already rows [0, M)
     Lease y(&c->scratch, st);                             // gather the groups of u rows through the scratch buffer
     CUDA_TRY(y.acquire(M * pitch * sizeof(uint32_t)));
@@ -337,10 +324,9 @@ int run_aligned_asym_mixed(Context* c, uint32_t* x, size_t N, size_t M, size_t s
 template <class Transform>
 int run_repacked(Context* c, uint32_t* d, size_t N, size_t rows_back, size_t size, size_t pitch, cudaStream_t st, Transform transform)
 {
-    const bool aligned = (pitch % 4 == 0) && (((uintptr_t)d) % 16 == 0);
-    if (aligned) return transform(d, pitch);
+    if (is_aligned(d, pitch)) return transform(d, pitch);
     // unaligned layout: repack into a padded copy, transform, copy the SIZE data words back
-    const size_t ppitch = (size + 3) / 4 * 4;
+    const size_t ppitch = padded_pitch(size);
     Lease pk(&c->packed, st);
     CUDA_TRY(pk.acquire(N * ppitch * sizeof(uint32_t)));
     CUDA_TRY(launch_pack(d, pitch, pk.ptr(), ppitch, N, (uint32_t)size, st)); g_launches++;
@@ -349,14 +335,27 @@ int run_repacked(Context* c, uint32_t* d, size_t N, size_t rows_back, size_t siz
     return 0;
 }
 
-int run_dev(uint32_t* d, size_t N, size_t size, size_t pitch, int mode, void* stream, const char* who, PassTimer* timer = nullptr)
+// The device entry points, validated in full before anything is allocated or launched.  Unaligned layouts are repacked
+// (run_repacked), except where `repack_ok` is false: there they are rejected.
+int ntt_dev(uint32_t* d, size_t N, size_t size, size_t pitch, bool inverse, void* stream, const char* who)
 {
     Context* c = ctx(who);
     if (!c) return FASTECC_B200_ENOINIT;
-    if (int rc = check_shape(N, size, mode >= 2 ? FASTECC_B200_MAX_LOG_N_ENCODE : FASTECC_B200_MAX_LOG_N, who, mode != 2)) return rc;
     if (int rc = check_rows(d, N, size, pitch, false, who)) return rc;
+    if (int rc = check_order(N, N, size, is_aligned(d, pitch) ? pitch : padded_pitch(size), FASTECC_B200_MAX_LOG_N, true, who)) return rc;
     cudaStream_t st = (cudaStream_t)stream;
-    return run_repacked(c, d, N, N, size, pitch, st, [&](uint32_t* x, size_t p) { return run_aligned(c, x, N, size, p, mode, st, timer); });
+    return run_repacked(c, d, N, N, size, pitch, st, [&](uint32_t* x, size_t p) { return ntt(c, x, N, size, p, inverse, st); });
+}
+
+int encode_dev(uint32_t* d, size_t N, size_t M, size_t size, size_t pitch, void* stream, bool mixed_ok, bool repack_ok, const char* who,
+               PassTimer* timer = nullptr)
+{
+    Context* c = ctx(who);
+    if (!c) return FASTECC_B200_ENOINIT;
+    if (int rc = check_rows(d, N, size, pitch, !repack_ok, who)) return rc;
+    if (int rc = check_order(N, M, size, is_aligned(d, pitch) ? pitch : padded_pitch(size), FASTECC_B200_MAX_LOG_N_ENCODE, mixed_ok, who)) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    return run_repacked(c, d, N, M, size, pitch, st, [&](uint32_t* x, size_t p) { return encode(c, x, N, M, size, p, st, timer); });
 }
 
 // The host (T**) entry points: the N blocks are staged in a padded device copy, `transform(x, SIZE, pitch)` runs on it in place
@@ -367,7 +366,7 @@ int run_host(Context* c, uint32_t** data, size_t N, size_t rows_back, size_t siz
     if (!data) return fail(FASTECC_B200_EINVAL, "%s: null block table", who);
     for (size_t i = 0; i < N; i++) if (!data[i]) return fail(FASTECC_B200_EINVAL, "%s: data[%zu] is null", who, i);
     std::lock_guard<std::mutex> host_lock(g_host_mu);
-    const size_t pitch = (size + 3) / 4 * 4;
+    const size_t pitch = padded_pitch(size);
     CUDA_TRY(c->staging.reserve(N * pitch * sizeof(uint32_t)));
     uint32_t* dv = (uint32_t*)c->staging.p;
     cudaStream_t st = c->stream;
@@ -406,12 +405,21 @@ int run_host(Context* c, uint32_t** data, size_t N, size_t rows_back, size_t siz
     return 0;
 }
 
-int run_host_mode(uint32_t** data, size_t N, size_t size, int mode, const char* who)
+// The host entry points, validated as the device ones (at the pitch of the staged copy) before anything is staged.
+int ntt_host(uint32_t** data, size_t N, size_t size, bool inverse, const char* who)
 {
     Context* c = ctx(who);
     if (!c) return FASTECC_B200_ENOINIT;
-    if (int rc = check_shape(N, size, mode >= 2 ? FASTECC_B200_MAX_LOG_N_ENCODE : FASTECC_B200_MAX_LOG_N, who, mode != 2)) return rc;
-    return run_host(c, data, N, N, size, who, [&](uint32_t* x, size_t w, size_t pitch) { return run_aligned(c, x, N, w, pitch, mode, c->stream); });
+    if (int rc = check_order(N, N, size, padded_pitch(size), FASTECC_B200_MAX_LOG_N, true, who)) return rc;
+    return run_host(c, data, N, N, size, who, [&](uint32_t* x, size_t w, size_t pitch) { return ntt(c, x, N, w, pitch, inverse, c->stream); });
+}
+
+int encode_host(uint32_t** data, size_t N, size_t M, size_t size, bool mixed_ok, const char* who)
+{
+    Context* c = ctx(who);
+    if (!c) return FASTECC_B200_ENOINIT;
+    if (int rc = check_order(N, M, size, padded_pitch(size), FASTECC_B200_MAX_LOG_N_ENCODE, mixed_ok, who)) return rc;
+    return run_host(c, data, N, M, size, who, [&](uint32_t* x, size_t w, size_t pitch) { return encode(c, x, N, M, w, pitch, c->stream); });
 }
 
 // One pass of a sharded encode / transform (the three fastecc_b200_*_shard_pass* entry points): kShard (exchange by the
@@ -498,17 +506,17 @@ int fastecc_b200_num_sms(void) { return g_ctx ? g_ctx->num_sms : 0; }
 unsigned long long fastecc_b200_kernel_launches(void) { return g_launches.load(); }
 
 int fastecc_b200_ntt_u32_dev(uint32_t* d, size_t N, size_t size, size_t pitch, int inverse, void* stream)
-{ return run_dev(d, N, size, pitch, inverse ? 1 : 0, stream, "fastecc_b200_ntt_u32_dev"); }
+{ return ntt_dev(d, N, size, pitch, inverse != 0, stream, "fastecc_b200_ntt_u32_dev"); }
 
 int fastecc_b200_rs_encode_dev(uint32_t* d, size_t N, size_t size, size_t pitch, void* stream)
-{ return run_dev(d, N, size, pitch, 2, stream, "fastecc_b200_rs_encode_dev"); }
+{ return encode_dev(d, N, N, size, pitch, stream, false, true, "fastecc_b200_rs_encode_dev"); }
 
 int fastecc_b200_rs_encode_dev_timed(uint32_t* d, size_t N, size_t size, size_t pitch, void* stream, float* pass_ms, const char** pass_kernel, int* n_passes)
 {
     const char* who = "fastecc_b200_rs_encode_dev_timed";
     if (!pass_ms || !n_passes || *n_passes < 1) return fail(FASTECC_B200_EINVAL, "%s: pass_ms / n_passes missing", who);
     PassTimer t;
-    int rc = run_dev(d, N, size, pitch, 2, stream, who, &t);
+    int rc = encode_dev(d, N, N, size, pitch, stream, false, true, who, &t);
     if (rc == 0 && cudaStreamSynchronize((cudaStream_t)stream) != cudaSuccess) rc = fail(FASTECC_B200_ECUDA, "%s: %s", who, cudaGetErrorString(cudaGetLastError()));
     int n = 0;
     for (size_t i = 0; rc == 0 && i + 1 < t.ev.size() && n < *n_passes; ++i, ++n) {
@@ -586,23 +594,10 @@ int fastecc_b200_gfp_to_bytes_dev(const uint32_t* d_words, void* d_bytes, size_t
 }
 
 int fastecc_b200_rs_encode_asym_dev(uint32_t* d, size_t N, size_t M, size_t size, size_t pitch, void* stream)
-{
-    const char* who = "fastecc_b200_rs_encode_asym_dev";
-    Context* c = ctx(who);
-    if (!c) return FASTECC_B200_ENOINIT;
-    if (int rc = check_asym_shape(N, M, size, who)) return rc;
-    if (int rc = check_rows(d, N, size, pitch, true, who)) return rc;
-    return run_aligned_asym(c, d, N, M, size, pitch, (cudaStream_t)stream);
-}
+{ return encode_dev(d, N, M, size, pitch, stream, false, false, "fastecc_b200_rs_encode_asym_dev"); }
 
 int fastecc_b200_rs_encode_asym(uint32_t** data, size_t N, size_t M, size_t size)
-{
-    const char* who = "fastecc_b200_rs_encode_asym";
-    Context* c = ctx(who);
-    if (!c) return FASTECC_B200_ENOINIT;
-    if (int rc = check_asym_shape(N, M, size, who)) return rc;
-    return run_host(c, data, N, M, size, who, [&](uint32_t* x, size_t w, size_t pitch) { return run_aligned_asym(c, x, N, M, w, pitch, c->stream); });
-}
+{ return encode_host(data, N, M, size, false, "fastecc_b200_rs_encode_asym"); }
 
 int fastecc_b200_rs_encode_shard_pass(uint32_t* d_local, size_t N, int n_ranks, int rank, size_t size, size_t pitch, int which, void* stream)
 { return shard_pass(kShard, d_local, nullptr, N, n_ranks, rank, size, pitch, 0, which, stream, "fastecc_b200_rs_encode_shard_pass"); }
@@ -683,37 +678,22 @@ int fastecc_b200_ipc_close(void* d_ptr)
 }
 
 int fastecc_b200_ntt_u32(uint32_t** data, size_t N, size_t size, int inverse)
-{ return run_host_mode(data, N, size, inverse ? 1 : 0, "fastecc_b200_ntt_u32"); }
+{ return ntt_host(data, N, size, inverse != 0, "fastecc_b200_ntt_u32"); }
 
 int fastecc_b200_rs_encode(uint32_t** data, size_t N, size_t size)
-{ return run_host_mode(data, N, size, 2, "fastecc_b200_rs_encode"); }
+{ return encode_host(data, N, N, size, false, "fastecc_b200_rs_encode"); }
 
 int fastecc_b200_rs_encode_mixed(uint32_t** data, size_t N, size_t size)
-{ return run_host_mode(data, N, size, 3, "fastecc_b200_rs_encode_mixed"); }
+{ return encode_host(data, N, N, size, true, "fastecc_b200_rs_encode_mixed"); }
 
 int fastecc_b200_rs_encode_mixed_dev(uint32_t* d, size_t N, size_t size, size_t pitch, void* stream)
-{ return run_dev(d, N, size, pitch, 3, stream, "fastecc_b200_rs_encode_mixed_dev"); }
+{ return encode_dev(d, N, N, size, pitch, stream, true, true, "fastecc_b200_rs_encode_mixed_dev"); }
 
 int fastecc_b200_rs_encode_asym_mixed_dev(uint32_t* d, size_t N, size_t M, size_t size, size_t pitch, void* stream)
-{
-    const char* who = "fastecc_b200_rs_encode_asym_mixed_dev";
-    Context* c = ctx(who);
-    if (!c) return FASTECC_B200_ENOINIT;
-    if (int rc = check_rows(d, N, size, pitch, false, who)) return rc;
-    const bool aligned = (pitch % 4 == 0) && (((uintptr_t)d) % 16 == 0);
-    if (int rc = check_asym_mixed_shape(N, M, size, aligned ? pitch : (size + 3) / 4 * 4, who)) return rc;
-    cudaStream_t st = (cudaStream_t)stream;
-    return run_repacked(c, d, N, M, size, pitch, st, [&](uint32_t* x, size_t p) { return run_aligned_asym_mixed(c, x, N, M, size, p, st); });
-}
+{ return encode_dev(d, N, M, size, pitch, stream, true, true, "fastecc_b200_rs_encode_asym_mixed_dev"); }
 
 int fastecc_b200_rs_encode_asym_mixed(uint32_t** data, size_t N, size_t M, size_t size)
-{
-    const char* who = "fastecc_b200_rs_encode_asym_mixed";
-    Context* c = ctx(who);
-    if (!c) return FASTECC_B200_ENOINIT;
-    if (int rc = check_asym_mixed_shape(N, M, size, (size + 3) / 4 * 4, who)) return rc;
-    return run_host(c, data, N, M, size, who, [&](uint32_t* x, size_t w, size_t pitch) { return run_aligned_asym_mixed(c, x, N, M, w, pitch, c->stream); });
-}
+{ return encode_host(data, N, M, size, true, "fastecc_b200_rs_encode_asym_mixed"); }
 
 int fastecc_b200_pin_host_buffers(int enable)
 {

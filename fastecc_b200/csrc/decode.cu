@@ -13,6 +13,7 @@
 // data blocks (fastecc_b200_rs_decode_pattern_mixed, DESIGN 3c / 3e) use the same steps with rho = GF_Root(2N) split by the CRT.
 #include "../../include/fastecc_b200.h"
 #include "gf.cuh"
+#include "mixed_radix.h"
 #include <cuda_runtime.h>
 #include <vector>
 #include <new>
@@ -155,14 +156,11 @@ int build_pattern(fastecc_b200_erasures* E, const uint32_t* erased, cudaStream_t
     const size_t n2 = E->n2, me = E->me;
     const uint4* tw = context_power_table();
     LeafRoots lr{};
-    lr.r = (uint32_t)(n2 % 9 == 0 ? 9 : n2 % 3 == 0 ? 3 : 1);
-    const uint32_t p2 = (uint32_t)(n2 / lr.r);                                  // the power-of-two part, <= 2^20
-    uint32_t log_p2 = 0; while ((1u << log_p2) < p2) ++log_p2;
-    lr.log_step = gf::LOG_M - log_p2; lr.mask = p2 - 1; lr.b2 = 1;
+    const Order o = split_order(n2);                                            // n2 = r * 2^t, 2^t <= 2^20
+    const CrtSplit ab = crt_split(o.r, o.log2_m);
+    lr.r = o.r; lr.a2 = ab.a; lr.b2 = ab.b;
+    lr.log_step = gf::LOG_M - o.log2_m; lr.mask = (1u << o.log2_m) - 1;
     if (lr.r > 1) {
-        for (uint32_t a = 0; a < lr.r; ++a) if ((uint64_t)a * (p2 % lr.r) % lr.r == 1) { lr.a2 = a; break; }
-        uint64_t b = 1; for (uint32_t i = 0; i < log_p2; ++i) b = (b * (2 - (lr.r * b) % p2 + p2)) % p2;      // Newton: r*b = 1 mod 2^t
-        lr.b2 = (uint32_t)b;
         const uint32_t zr = gf::root(lr.r);
         for (uint32_t j = 0; j < 9; ++j) lr.zeta[j] = gf::powmod(zr, j);
     }
@@ -217,11 +215,10 @@ int make_pattern(size_t n_rows, const uint32_t* erased, size_t n_erased, void* s
     if (!out) return fail(FASTECC_B200_EINVAL, "%s: null output", who);
     *out = nullptr;
     if (!fecc::context_power_table()) return fail(FASTECC_B200_ENOINIT, "%s: call fastecc_b200_init() first", who);
-    if (!mixed && (n_rows < 2 || (n_rows & (n_rows - 1)) || n_rows > ((size_t)1 << FASTECC_B200_MAX_LOG_N)))
-        return fail(FASTECC_B200_EINVAL, "%s: the code word must have 2N = 2 .. 2^20 rows (a power of two), got %zu", who, n_rows);
-    const size_t r = n_rows % 9 == 0 ? 9 : n_rows % 3 == 0 ? 3 : 1, p2 = n_rows / r;     // n_rows = r * p2
-    if (mixed && (p2 < 2 || (p2 & (p2 - 1)) || p2 > ((size_t)1 << FASTECC_B200_MAX_LOG_N)))
-        return fail(FASTECC_B200_EINVAL, "%s: the code word must have 2N = 2^k, 3 * 2^k or 9 * 2^k rows, 1 <= k <= 20, got %zu", who, n_rows);
+    const Order o = split_order(n_rows);                                        // n_rows = r * 2^k
+    if (!o.r || (!mixed && o.r != 1) || o.log2_m < 1 || o.log2_m > FASTECC_B200_MAX_LOG_N)
+        return fail(FASTECC_B200_EINVAL, mixed ? "%s: the code word must have 2N = 2^k, 3 * 2^k or 9 * 2^k rows, 1 <= k <= 20, got %zu"
+                                               : "%s: the code word must have 2N = 2 .. 2^20 rows (a power of two), got %zu", who, n_rows);
     if (n_erased > n_rows / 2) return fail(FASTECC_B200_EINVAL, "%s: at most N = %zu of the 2N rows can be erased, got %zu", who, n_rows / 2, n_erased);
     if (n_erased && !erased) return fail(FASTECC_B200_EINVAL, "%s: null position list", who);
     for (size_t i = 0; i < n_erased; ++i)

@@ -59,37 +59,26 @@ __global__ void __launch_bounds__(256) radix_pass_kernel(const uint4* __restrict
     const size_t total = (size_t)M * s4;
     for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
         const uint32_t k2 = (uint32_t)(i / s4), c = (uint32_t)(i - (size_t)k2 * s4);
-        uint32_t f[R][4];
+        uint32_t f[4][R];
 #pragma unroll
         for (int n1 = 0; n1 < R; ++n1) {
             const uint4 v = src[((size_t)R * k2 + n1) * pitch4 + c];
-            f[n1][0] = v.x; f[n1][1] = v.y; f[n1][2] = v.z; f[n1][3] = v.w;
+            f[0][n1] = v.x; f[1][n1] = v.y; f[2][n1] = v.z; f[3][n1] = v.w;
             const unsigned long long e = (unsigned long long)n1 * k2;
             const uint32_t er = (uint32_t)((a_inv * (e % R)) % R); uint32_t em = (uint32_t)(((unsigned long long)b_inv * (e & (M - 1))) & (M - 1));
             if (inverse) em = (M - em) & (M - 1);                               // the power table is forward; C.zeta already has the direction
             const uint4 t = tw[(size_t)em << (20 - log_m)];                    // GF_Root(M)^(+-em)
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
-                uint32_t x = gf::canon(gf::mul(f[n1][j], t.x, t.y, t.z));      // inputs are taken mod P
-                f[n1][j] = er ? mulc(x, C.zeta[er]) : x;
+                uint32_t x = gf::canon(gf::mul(f[j][n1], t.x, t.y, t.z));      // inputs are taken mod P
+                f[j][n1] = er ? mulc(x, C.zeta[er]) : x;
             }
         }
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            if (R == 3) {
-                dft3(f[0][j], f[1][j], f[2][j], C);
-            } else {                                                            // 3 x 3 four-step, as the reference's NTT9 (ntt.cpp:114-146)
-                dft3(f[0][j], f[3][j], f[6][j], C); dft3(f[1][j], f[4][j], f[7][j], C); dft3(f[2][j], f[5][j], f[8][j], C);
-                f[4][j] = mulc(f[4][j], C.zeta[1]); f[5][j] = mulc(f[5][j], C.zeta[2]);
-                f[7][j] = mulc(f[7][j], C.zeta[2]); f[8][j] = mulc(f[8][j], C.zeta[4]);
-                dft3(f[0][j], f[1][j], f[2][j], C); dft3(f[3][j], f[4][j], f[5][j], C); dft3(f[6][j], f[7][j], f[8][j], C);
-            }
-        }
+        for (int j = 0; j < 4; ++j) dft_r<R>(f[j], C);
 #pragma unroll
-        for (int k1 = 0; k1 < R; ++k1) {
-            const int p = R == 3 ? k1 : (k1 % 3) * 3 + k1 / 3;                  // the 3 x 3 transpose: X[k1] sits at position 3*(k1 % 3) + k1 / 3
-            dst[((size_t)k2 + (size_t)M * k1) * pitch4 + c] = make_uint4(f[p][0], f[p][1], f[p][2], f[p][3]);
-        }
+        for (int k1 = 0; k1 < R; ++k1)
+            dst[((size_t)k2 + (size_t)M * k1) * pitch4 + c] = make_uint4(f[0][k1], f[1][k1], f[2][k1], f[3][k1]);
     }
 }
 
@@ -106,19 +95,23 @@ static void fill_codelets(RadixConsts& C, uint32_t r, bool inverse)
     fill3(C.c2, gf::mulmod((uint32_t)(((uint64_t)x1 + gf::P - x2) % gf::P), inv2));
 }
 
+// grid of the grid-stride radix kernels: one thread per item, at most 16 blocks of 256 per SM
+static unsigned grid_for(size_t total, int num_sms)
+{
+    return (unsigned)((total + 255) / 256 < (size_t)num_sms * 16 ? (total + 255) / 256 : (size_t)num_sms * 16);
+}
+
+// The launchers take what api.cu has validated: r in {3, 9} (s | r for the fold), M a power of two.
 cudaError_t launch_radix_pass(const uint32_t* src, uint32_t* dst, uint32_t pitch4, uint32_t s4, uint32_t r, uint32_t M, bool inverse, const uint4* tw, int num_sms, cudaStream_t st)
 {
-    if ((r != 3 && r != 9) || !M || (M & (M - 1)) || M > gf::M) return cudaErrorInvalidValue;
+    auto kernel = r == 3 ? radix_pass_kernel<3> : r == 9 ? radix_pass_kernel<9> : nullptr;
+    if (!kernel || !M || (M & (M - 1)) || M > gf::M) return cudaErrorInvalidValue;
     uint32_t log_m = 0; while ((1u << log_m) < M) ++log_m;
     RadixConsts C;
     fill_codelets(C, r, inverse);
-    uint32_t a_inv = 0, b_inv = 0;                                              // a = M^-1 mod r, b = r^-1 mod M
-    for (uint32_t a = 0; a < r; ++a) if (((uint64_t)a * (M % r)) % r == 1 % r) { a_inv = a; break; }
-    if (M > 1) { uint64_t b = 1; for (uint32_t i = 0; i < log_m; ++i) b = (b * (2 - (r * b) % M + M)) % M; b_inv = (uint32_t)b; }     // Newton: r*b = 1 mod 2^k
-    const size_t total = (size_t)M * s4;
-    const unsigned grid = (unsigned)((total + 255) / 256 < (size_t)num_sms * 16 ? (total + 255) / 256 : (size_t)num_sms * 16);
-    if (r == 3) radix_pass_kernel<3><<<grid, 256, 0, st>>>(reinterpret_cast<const uint4*>(src), reinterpret_cast<uint4*>(dst), pitch4, s4, M, log_m, a_inv, b_inv, inverse ? 1 : 0, C, tw);
-    else        radix_pass_kernel<9><<<grid, 256, 0, st>>>(reinterpret_cast<const uint4*>(src), reinterpret_cast<uint4*>(dst), pitch4, s4, M, log_m, a_inv, b_inv, inverse ? 1 : 0, C, tw);
+    const CrtSplit ab = crt_split(r, log_m);                                   // a = M^-1 mod r, b = r^-1 mod M
+    kernel<<<grid_for((size_t)M * s4, num_sms), 256, 0, st>>>(reinterpret_cast<const uint4*>(src), reinterpret_cast<uint4*>(dst), pitch4, s4, M, log_m, ab.a, ab.b,
+                                                             inverse ? 1 : 0, C, tw);
     return cudaGetLastError();
 }
 
@@ -139,6 +132,31 @@ struct EncodeConsts {
 };
 
 template <int R>
+__device__ __forceinline__ void encode_codelets(const uint4* row, uint32_t pitch4, uint32_t k2, uint32_t mask, uint32_t sh, uint32_t a2, uint32_t b2,
+                                                const EncodeConsts& C, const uint4* __restrict__ tw, uint32_t (&f)[4][R])
+{
+    const uint32_t k2r = k2 % R;
+#pragma unroll
+    for (int n1 = 0; n1 < R; ++n1) {
+        const uint4 v = row[(size_t)n1 * pitch4];
+        const uint32_t cr = (uint32_t)(((1 - 2 * n1) % R + R) % R);
+        const uint32_t er = (a2 * ((k2r * cr) % R)) % R, em = (b2 * (k2 * (uint32_t)(1 - 2 * n1))) & mask;
+        const uint4 t = tw[(size_t)em << sh];
+        f[0][n1] = mulc(gf::canon(gf::mul(v.x, t.x, t.y, t.z)), C.zin[er]);
+        f[1][n1] = mulc(gf::canon(gf::mul(v.y, t.x, t.y, t.z)), C.zin[er]);
+        f[2][n1] = mulc(gf::canon(gf::mul(v.z, t.x, t.y, t.z)), C.zin[er]);
+        f[3][n1] = mulc(gf::canon(gf::mul(v.w, t.x, t.y, t.z)), C.zin[er]);
+    }
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        dft_r<R>(f[j], C.inv);
+#pragma unroll
+        for (int k1 = 1; k1 < R; ++k1) f[j][k1] = mulc(f[j][k1], C.sigma[k1]);
+        dft_r<R>(f[j], C.fwd);
+    }
+}
+
+template <int R>
 __global__ void __launch_bounds__(256) radix_encode_kernel(uint4* __restrict__ x, uint32_t pitch4, uint32_t s4, uint32_t M, uint32_t log_m,
                                                            uint32_t a2, uint32_t b2, EncodeConsts C, const uint4* __restrict__ tw)
 {
@@ -148,24 +166,7 @@ __global__ void __launch_bounds__(256) radix_encode_kernel(uint4* __restrict__ x
         const uint32_t k2 = (uint32_t)(i / s4), c = (uint32_t)(i - (size_t)k2 * s4), k2r = k2 % R;
         uint4* row = x + (size_t)R * k2 * pitch4 + c;
         uint32_t f[4][R];
-#pragma unroll
-        for (int n1 = 0; n1 < R; ++n1) {
-            const uint4 v = row[(size_t)n1 * pitch4];
-            const uint32_t cr = (uint32_t)(((1 - 2 * n1) % R + R) % R);         // 1 - 2*n1 mod r
-            const uint32_t er = (a2 * ((k2r * cr) % R)) % R, em = (b2 * (k2 * (uint32_t)(1 - 2 * n1))) & mask;
-            const uint4 t = tw[(size_t)em << sh];
-            f[0][n1] = mulc(gf::canon(gf::mul(v.x, t.x, t.y, t.z)), C.zin[er]);
-            f[1][n1] = mulc(gf::canon(gf::mul(v.y, t.x, t.y, t.z)), C.zin[er]);
-            f[2][n1] = mulc(gf::canon(gf::mul(v.z, t.x, t.y, t.z)), C.zin[er]);
-            f[3][n1] = mulc(gf::canon(gf::mul(v.w, t.x, t.y, t.z)), C.zin[er]);
-        }
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            dft_r<R>(f[j], C.inv);
-#pragma unroll
-            for (int k1 = 1; k1 < R; ++k1) f[j][k1] = mulc(f[j][k1], C.sigma[k1]);
-            dft_r<R>(f[j], C.fwd);
-        }
+        encode_codelets<R>(row, pitch4, k2, mask, sh, a2, b2, C, tw, f);
         row[0] = make_uint4(f[0][0], f[1][0], f[2][0], f[3][0]);                 // j1 = 0: twiddle 1
 #pragma unroll
         for (int j1 = 1; j1 < R; ++j1) {
@@ -182,22 +183,24 @@ __global__ void __launch_bounds__(256) radix_encode_kernel(uint4* __restrict__ x
     }
 }
 
-cudaError_t launch_radix_encode(uint32_t* x, uint32_t pitch4, uint32_t s4, uint32_t r, uint32_t M, const uint4* tw, int num_sms, cudaStream_t st)
+// The constants of both step-2 kernels of the encode of N = r * M blocks; returns {a2, b2} = {(2M)^-1 mod r, r^-1 mod 2M}.
+static CrtSplit fill_encode(EncodeConsts& C, uint32_t r, uint32_t M, uint32_t log_m)
 {
-    if ((r != 3 && r != 9) || !M || (M & (M - 1)) || M > gf::M / 2) return cudaErrorInvalidValue;
-    uint32_t log_m = 0; while ((1u << log_m) < M) ++log_m;
-    EncodeConsts C;
     fill_codelets(C.inv, r, true);
     fill_codelets(C.fwd, r, false);
     const uint32_t zr = gf::powmod(gf::GEN, (gf::P - 1) / r), sigma = gf::powmod(gf::GEN, (gf::P - 1) / (2 * r)), inv_n = gf::inv(r * M);
     for (uint32_t j = 0; j < 9; ++j) { fill3(C.zin[j], gf::mulmod(gf::powmod(zr, j), inv_n)); fill3(C.sigma[j], gf::powmod(sigma, j)); }
-    uint32_t a2 = 0;                                                            // a2 = (2M)^-1 mod r, b2 = r^-1 mod 2M
-    for (uint32_t a = 0; a < r; ++a) if (((uint64_t)a * ((2 * M) % r)) % r == 1) { a2 = a; break; }
-    uint64_t b2 = 1; for (uint32_t i = 0; i <= log_m; ++i) b2 = (b2 * (2 - (r * b2) % (2 * M) + 2 * M)) % (2 * M);     // Newton: r*b = 1 mod 2^(k+1)
-    const size_t total = (size_t)M * s4;
-    const unsigned grid = (unsigned)((total + 255) / 256 < (size_t)num_sms * 16 ? (total + 255) / 256 : (size_t)num_sms * 16);
-    if (r == 3) radix_encode_kernel<3><<<grid, 256, 0, st>>>(reinterpret_cast<uint4*>(x), pitch4, s4, M, log_m, a2, (uint32_t)b2, C, tw);
-    else        radix_encode_kernel<9><<<grid, 256, 0, st>>>(reinterpret_cast<uint4*>(x), pitch4, s4, M, log_m, a2, (uint32_t)b2, C, tw);
+    return crt_split(r, log_m + 1);
+}
+
+cudaError_t launch_radix_encode(uint32_t* x, uint32_t pitch4, uint32_t s4, uint32_t r, uint32_t M, const uint4* tw, int num_sms, cudaStream_t st)
+{
+    auto kernel = r == 3 ? radix_encode_kernel<3> : r == 9 ? radix_encode_kernel<9> : nullptr;
+    if (!kernel || !M || (M & (M - 1)) || M > gf::M / 2) return cudaErrorInvalidValue;
+    uint32_t log_m = 0; while ((1u << log_m) < M) ++log_m;
+    EncodeConsts C;
+    const CrtSplit ab = fill_encode(C, r, M, log_m);
+    kernel<<<grid_for((size_t)M * s4, num_sms), 256, 0, st>>>(reinterpret_cast<uint4*>(x), pitch4, s4, M, log_m, ab.a, ab.b, C, tw);
     return cudaGetLastError();
 }
 
@@ -232,24 +235,7 @@ __global__ void __launch_bounds__(256) radix_fold_kernel(uint4* __restrict__ x, 
             const uint32_t k2 = t + (q << log_t), k2r = k2 % R;
             const uint4* row = x + (size_t)R * k2 * pitch4 + c;
             uint32_t f[4][R];
-#pragma unroll
-            for (int n1 = 0; n1 < R; ++n1) {                                    // as radix_encode_kernel
-                const uint4 v = row[(size_t)n1 * pitch4];
-                const uint32_t cr = (uint32_t)(((1 - 2 * n1) % R + R) % R);
-                const uint32_t er = (a2 * ((k2r * cr) % R)) % R, em = (b2 * (k2 * (uint32_t)(1 - 2 * n1))) & mask;
-                const uint4 w = tw[(size_t)em << sh];
-                f[0][n1] = mulc(gf::canon(gf::mul(v.x, w.x, w.y, w.z)), C.e.zin[er]);
-                f[1][n1] = mulc(gf::canon(gf::mul(v.y, w.x, w.y, w.z)), C.e.zin[er]);
-                f[2][n1] = mulc(gf::canon(gf::mul(v.z, w.x, w.y, w.z)), C.e.zin[er]);
-                f[3][n1] = mulc(gf::canon(gf::mul(v.w, w.x, w.y, w.z)), C.e.zin[er]);
-            }
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                dft_r<R>(f[j], C.e.inv);
-#pragma unroll
-                for (int k1 = 1; k1 < R; ++k1) f[j][k1] = mulc(f[j][k1], C.e.sigma[k1]);
-                dft_r<R>(f[j], C.e.fwd);                                        // outputs j1 != 0 mod S are dead code
-            }
+            encode_codelets<R>(row, pitch4, k2, mask, sh, a2, b2, C.e, tw, f);
 #pragma unroll
             for (int j = 0; j < 4; ++j) acc[0][j] = addm(acc[0][j], f[j][0]);  // u = 0: J = 0, twiddle 1
 #pragma unroll
@@ -272,37 +258,23 @@ __global__ void __launch_bounds__(256) radix_fold_kernel(uint4* __restrict__ x, 
 cudaError_t launch_radix_fold(uint32_t* x, uint32_t pitch4, uint32_t s4, uint32_t r, uint32_t M, uint32_t s, uint32_t log_d2, uint32_t log_fold,
                               const uint4* tw, int num_sms, cudaStream_t st)
 {
-    if ((r != 3 && r != 9) || !M || (M & (M - 1)) || M > gf::M / 2 || (s != 1 && s != 3 && s != 9) || r % s || (M >> log_d2) == 0 || log_fold > log_d2)
-        return cudaErrorInvalidValue;
+    auto kernel = r == 3 ? (s == 1 ? radix_fold_kernel<3, 1> : s == 3 ? radix_fold_kernel<3, 3> : nullptr)
+                : r == 9 ? (s == 1 ? radix_fold_kernel<9, 1> : s == 3 ? radix_fold_kernel<9, 3> : s == 9 ? radix_fold_kernel<9, 9> : nullptr) : nullptr;
+    if (!kernel || !M || (M & (M - 1)) || M > gf::M / 2 || (M >> log_d2) == 0 || log_fold > log_d2) return cudaErrorInvalidValue;
     uint32_t log_m = 0; while ((1u << log_m) < M) ++log_m;
     FoldConsts C;
-    fill_codelets(C.e.inv, r, true);
-    fill_codelets(C.e.fwd, r, false);
-    const uint32_t zr = gf::powmod(gf::GEN, (gf::P - 1) / r), sigma = gf::powmod(gf::GEN, (gf::P - 1) / (2 * r)), inv_n = gf::inv(r * M);
-    for (uint32_t j = 0; j < 9; ++j) { fill3(C.e.zin[j], gf::mulmod(gf::powmod(zr, j), inv_n)); fill3(C.e.sigma[j], gf::powmod(sigma, j)); }
-    uint32_t a2 = 0;                                                            // a2 = (2M)^-1 mod r, b2 = r^-1 mod 2M
-    for (uint32_t a = 0; a < r; ++a) if (((uint64_t)a * ((2 * M) % r)) % r == 1) { a2 = a; break; }
-    uint64_t b2 = 1; for (uint32_t i = 0; i <= log_m; ++i) b2 = (b2 * (2 - (r * b2) % (2 * M) + 2 * M)) % (2 * M);
-    const uint64_t d2 = 1ull << log_d2, D = s * d2;
-    uint64_t rinv = 1; for (uint32_t i = 0; i < log_d2; ++i) rinv = (rinv * (2 - (r * rinv) % d2 + d2)) % d2;   // r^-1 mod 2^i
+    const CrtSplit ab = fill_encode(C.e, r, M, log_m);
+    const uint64_t d2 = 1ull << log_d2, D = s * d2, rinv = crt_split(r, log_d2).b;           // r^-1 mod 2^i
     for (uint32_t u = 0; u < 9; ++u) {
         C.tr[u] = C.tm[u] = C.d[u] = 0;
         if (u >= r / s) continue;
         const uint64_t j1 = (uint64_t)s * u, cj = (d2 - (j1 * rinv) % d2) % d2, J = j1 + r * cj;   // c_j1 = -j1 * r^-1 mod 2^i
-        C.tr[u] = (uint32_t)((2 * J % r) * a2 % r);
-        C.tm[u] = (uint32_t)((2 * J % (2 * M)) * b2 % (2 * M));
+        C.tr[u] = (uint32_t)((2 * J % r) * ab.a % r);
+        C.tm[u] = (uint32_t)((2 * J % (2 * M)) * ab.b % (2 * M));
         C.d[u] = (uint32_t)(J / D);
     }
     const uint32_t log_t = log_m - log_fold;
-    const size_t total = (size_t)s4 << log_t;
-    const unsigned grid = (unsigned)((total + 255) / 256 < (size_t)num_sms * 16 ? (total + 255) / 256 : (size_t)num_sms * 16);
-    uint4* x4 = reinterpret_cast<uint4*>(x);
-    const uint32_t nf = 1u << log_fold;
-    if      (r == 3 && s == 1) radix_fold_kernel<3, 1><<<grid, 256, 0, st>>>(x4, pitch4, s4, M, log_m, log_t, nf, a2, (uint32_t)b2, C, tw);
-    else if (r == 3)           radix_fold_kernel<3, 3><<<grid, 256, 0, st>>>(x4, pitch4, s4, M, log_m, log_t, nf, a2, (uint32_t)b2, C, tw);
-    else if (s == 1)           radix_fold_kernel<9, 1><<<grid, 256, 0, st>>>(x4, pitch4, s4, M, log_m, log_t, nf, a2, (uint32_t)b2, C, tw);
-    else if (s == 3)           radix_fold_kernel<9, 3><<<grid, 256, 0, st>>>(x4, pitch4, s4, M, log_m, log_t, nf, a2, (uint32_t)b2, C, tw);
-    else                       radix_fold_kernel<9, 9><<<grid, 256, 0, st>>>(x4, pitch4, s4, M, log_m, log_t, nf, a2, (uint32_t)b2, C, tw);
+    kernel<<<grid_for((size_t)s4 << log_t, num_sms), 256, 0, st>>>(reinterpret_cast<uint4*>(x), pitch4, s4, M, log_m, log_t, 1u << log_fold, ab.a, ab.b, C, tw);
     return cudaGetLastError();
 }
 

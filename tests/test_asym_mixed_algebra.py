@@ -1,5 +1,5 @@
 """CPU: the encode of N = r * L data blocks (r in {3, 9}, L = 2^k) into M | N parity blocks (csrc/mixed_radix.cu
-radix_fold_kernel between the power-of-two transforms, api.cu run_aligned_asym_mixed, DESIGN 3f) restated in plain Python
+radix_fold_kernel between the power-of-two transforms, api.cu encode, DESIGN 3f) restated in plain Python
 integers: the constants as launch_radix_fold computes them (the coset twist of the output twiddle and its CRT split, the
 output rows d_u), the kernel's fold by 2^f <= 2^i in place, the r / s forward transforms of order L / 2^f and the gather of
 every 2^(i-f)-th output -- checked against every (N/M)-th parity of the encode by definition, for every divisor M and every

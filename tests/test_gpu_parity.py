@@ -408,15 +408,16 @@ def test_argument_validation(fecc):
 
 def test_device_entry_point_argument_tables(fecc):
     """One table of argument tuples per device entry point that takes a row buffer: every rule of its validation, broken on
-    its own, must give FASTECC_B200_EINVAL (-1) before anything is launched, and the valid calls must give 0.  Every pointer
-    lies in ONE device allocation that covers rows x pitch of every tuple (the largest, at the 32-bit chunk-count limit, spans
-    2^36 bytes), so a tuple accepted by mistake stays inside it.  Not listed: the shard passes' upper pitch bound (their
-    smallest buffer at that pitch is 64 rows of 16 GiB) and the ENOINIT check (the session is initialised)."""
+    its own, must give FASTECC_B200_EINVAL (-1) before anything is launched (kernel_launches() does not move), and the valid
+    calls must give 0.  Every pointer lies in ONE device allocation that covers rows x pitch of every tuple (the largest, at
+    the 32-bit chunk-count limit, span 2^36 bytes and a little more), so a tuple accepted by mistake stays inside it.  Not
+    listed: the shard passes' upper pitch bound (their smallest buffer at that pitch is 64 rows of 16 GiB) and the ENOINIT
+    check (the session is initialised)."""
     import ctypes
     import torch
     L = fecc.lib()
     torch.cuda.empty_cache()
-    buf = torch.empty((1 << 34) + (1 << 21), dtype=torch.int32, device="cuda")     # 64 GiB + 8 MiB, never initialised
+    buf = torch.empty((1 << 34) + (1 << 24), dtype=torch.int32, device="cuda")     # 64 GiB + 64 MiB, never initialised
     B = buf.data_ptr()
     C = B + (1 << 36)                                                              # row constants of row_scale: past every row
     D = B + (1 << 30)                                                              # byte blocks of bytes_to_gfp
@@ -435,6 +436,8 @@ def test_device_entry_point_argument_tables(fecc):
             (bad, B, 1, MAXP + 1, BIG, 0), (bad, B, 3, MAXP + 1, BIG, 1),
             (bad, B, 16, 8, 4, 0), (bad, B, 1, 4, BIG, 0), (bad, B, 1, 4, MAXP + 1, 0),
             (bad, B, 1 << 20, 4, 1 << 14, 0), (bad, B, 1 << 20, 4, (1 << 14) - 3, 0),      # 2^20 x ceil(pitch / 4) = 2^32 chunks
+            (bad, B, 3, 4, MAXP, 0),                                                  # 3 rows of the largest pitch: r * pitch overflows
+            (bad, B + 4, 3, 1 << 31, (1 << 31) + 1, 0),                               # the same at the repacked pitch 2^31
             (good, B, 1 << 12, 64, 64, 0), (good, B, 1 << 12, 64, 64, 1), (good, B, 1 << 20, 4, 4, 0), (good, B, 48, 4, 4, 1),
             (good, B, 16, 5, 7, 0), (good, B + 4, 16, 4, 4, 0),                       # unaligned layouts are repacked
         ]),
@@ -452,6 +455,26 @@ def test_device_entry_point_argument_tables(fecc):
             (bad, B, 16, 4, 8, 4), (bad, B, 1, 1, 4, BIG), (bad, B, 16, 4, 4, 6), (bad, B + 4, 16, 4, 4, 4),
             (bad, B, 1 << 19, 1, 4, 1 << 15),
             (good, B, 1 << 12, 1 << 10, 64, 64), (good, B, 16, 4, 4, 4), (good, B, 1 << 19, 1 << 18, 4, 4),
+        ]),
+        "rs_encode_mixed_dev": (L.fastecc_b200_rs_encode_mixed_dev, [    # (d, N, SIZE, pitch)
+            *[(bad, B, N, 4, 4) for N in (0, 5, 15, 27, 45, 1 << 20, 3 << 20, 9 << 20)],
+            (bad, 0, 48, 4, 4), (bad, B, 48, 0, 4), (bad, B, 48, 8, 4), (bad, B, 3, 4, BIG), (bad, B, 3, MAXP + 1, BIG),
+            (bad, B, 3, 4, MAXP),                                                     # 3 rows of the largest pitch: r * pitch overflows
+            (bad, B + 4, 3, 1 << 31, (1 << 31) + 1),                                  # the same at the repacked pitch 2^31
+            (bad, B, 9 << 19, 4, 3644),                                               # 2^32 16-byte chunks or more
+            (good, B, 3, 4, 4), (good, B, 9, 1, 4), (good, B, 3 << 10, 8, 8), (good, B, 9 << 10, 64, 64), (good, B, 1 << 12, 16, 16),
+            (good, B, 3 << 19, 4, 4), (good, B, 9 << 19, 4, 4), (good, B, 48, 5, 7), (good, B + 4, 48, 4, 4),
+        ]),
+        "rs_encode_asym_mixed_dev": (L.fastecc_b200_rs_encode_asym_mixed_dev, [      # (d, N, M, SIZE, pitch)
+            *[(bad, B, N, 1, 4, 4) for N in (0, 5, 15, 27, 45, 1 << 20, 3 << 20, 9 << 20)],
+            (bad, B, 48, 0, 4, 4), (bad, B, 48, 49, 4, 4), (bad, B, 48, 96, 4, 4), (bad, B, 48, 5, 4, 4), (bad, B, 48, 9, 4, 4),
+            (bad, B, 3, 2, 4, 4), (bad, B, 9 << 19, 7, 4, 4), (bad, B, 1 << 10, 3, 4, 4),
+            (bad, 0, 48, 16, 4, 4), (bad, B, 48, 16, 0, 4), (bad, B, 48, 16, 8, 4), (bad, B, 3, 1, 4, BIG), (bad, B, 3, 1, MAXP + 1, BIG),
+            (bad, B, 3, 1, 4, MAXP),                                                  # 3 rows of the largest pitch: r * pitch overflows
+            (bad, B, 9 << 19, 9, 4, 3644),                                            # 2^32 16-byte chunks or more
+            (good, B, 3, 1, 4, 4), (good, B, 3, 3, 4, 4), (good, B, 9, 3, 1, 4), (good, B, 3 << 10, 1 << 10, 8, 8), (good, B, 9 << 10, 9, 64, 64),
+            (good, B, 1 << 12, 1 << 9, 16, 16), (good, B, 3 << 19, 1 << 10, 4, 4), (good, B, 9 << 19, 1, 4, 4), (good, B, 9 << 19, 9 << 19, 4, 4),
+            (good, B, 48, 12, 5, 7), (good, B + 4, 48, 6, 4, 4),
         ]),
         "row_scale_dev": (L.fastecc_b200_row_scale_dev, [    # (d, rows, SIZE, pitch, consts)
             (bad, 0, 16, 4, 4, C), (bad, B, 16, 4, 4, 0), (bad, B, 16, 0, 4, C),
@@ -509,9 +532,12 @@ def test_device_entry_point_argument_tables(fecc):
     wrong = []
     for name, (fn, cases) in tables.items():
         for kind, *args in cases:
+            launches = L.fastecc_b200_kernel_launches()
             rc = fn(*args, st)
             if rc != (0 if kind == good else -1):
                 wrong.append((name, args, rc, L.fastecc_b200_last_error().decode()))
+            if kind == bad and L.fastecc_b200_kernel_launches() != launches:           # rejected before anything is launched
+                wrong.append((name, args, "launched", L.fastecc_b200_kernel_launches() - launches))
     torch.cuda.synchronize()
     del buf
     torch.cuda.empty_cache()

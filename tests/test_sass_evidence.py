@@ -48,6 +48,20 @@ def test_headline_kernels_use_the_fp64_quotient_and_tma(sass, pattern):
     assert sum(1 for l in body if "LDL" in l or "STL" in l) <= 4                  # no spilling to speak of
 
 
+def test_radix_encode_kernel_is_in_the_library_and_does_not_spill(sass):
+    hits = {k: v for k, v in sass.items() if "radix_encode_kernel" in k}
+    assert sorted(re.search(r"ILi(\d)E", k).group(1) for k in hits) == ["3", "9"], list(hits)
+    for k, body in hits.items():
+        assert body and not any("LDL" in l or "STL" in l for l in body), k
+
+
+def test_radix_fold_kernel_is_in_the_library_and_does_not_spill(sass):
+    hits = {k: v for k, v in sass.items() if "radix_fold_kernel" in k}
+    assert sorted(re.search(r"ILi(\d)ELi(\d)E", k).groups() for k in hits) == [("3", "1"), ("3", "3"), ("9", "1"), ("9", "3"), ("9", "9")], list(hits)
+    for k, body in hits.items():
+        assert body and not any("LDL" in l or "STL" in l for l in body), k
+
+
 def test_library_contains_every_kernel_family(sass):
     names = " ".join(sass)
     for k in ("ntt_pass_kernel", "build_tables_kernel", "small_dft_kernel", "radix_pass_kernel", "row_scale_kernel", "shard_barrier_kernel",
