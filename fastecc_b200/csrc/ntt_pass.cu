@@ -3,7 +3,8 @@
 // the RS scaling (RS.cpp:51-59) and the start of the forward transform in a single pass.
 //
 // Execution model (DESIGN.md section 5): persistent CTAs of 256 threads, two per SM, each walking a sequence of
-// 64 KiB tiles (row set x column strip).  Per tile:
+// 64 KiB tiles (row set x column strip); the fused 1024-row pass instead runs one CTA of 512 threads per SM over 128 KiB
+// tiles with 128-byte rows (pass_threads() in ntt_tile.cuh).  Per tile:
 //   * one elected thread issues the TMA traffic: cp.async.bulk.tensor (3-D tensor map over [word][row-in-set][set],
 //     boxes of <= 256 rows) for the tile and, when the row set changes, one cp.async.bulk for the set's precomputed
 //     twiddle tables; completion is tracked by an mbarrier (expect_tx / complete_tx).  The next tile is requested
@@ -69,28 +70,31 @@ __device__ __forceinline__ bool tile_decode(const PassParams& P, uint32_t groups
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" :: "r"(smem_u32(bar)) : "memory"); }
 
 // LR / NXF / TMA are compile-time: the kernel patches them into its copy of the parameters, so every shift, stride
-// and placement branch in ntt_tile.cuh folds to an immediate (keeps the 64 data registers from spilling).
-template <int LR, int NXF, int TMA>
-__global__ void __launch_bounds__(kThreads, 2) ntt_pass_kernel(const PassParams Pin, const __grid_constant__ CUtensorMap tmap)
+// and placement branch in ntt_tile.cuh folds to an immediate (keeps the 64 data registers from spilling).  NT is the
+// geometry, pass_threads(LR, NXF, TMA): 256 threads (2 CTAs per SM, 64 KiB tiles) or 512 (1 CTA per SM, 128 KiB tiles);
+// either way 16 warps per SM at 128 registers.
+template <int LR, int NXF, int TMA, int NT>
+__global__ void __launch_bounds__(NT, NT == kWideThreads ? 1 : 2) ntt_pass_kernel(const PassParams Pin, const __grid_constant__ CUtensorMap tmap)
 {
     PassParams P = Pin;
     P.log_r = LR; P.nxf = NXF; P.use_tma = TMA != 0;
     if (TMA != 2) P.log_g = 0;                            // TMA == 2: the instantiation whose stores pick a destination GPU (sharded, §8)
     extern __shared__ __align__(1024) uint4 smem[];
     constexpr uint32_t R = 1u << LR;
-    uint4* tile = smem;                                   // 4096 chunks, natural row order
+    constexpr uint32_t kChunks = Geom<NT>::chunks;
+    uint4* tile = smem;                                   // kChunks chunks, natural row order
     // stage tables: a transform whose twist does not depend on the row set (t1 == 0) has ONE table, loaded once;
     // the others are double-buffered per set.  Slot of transform x in buffer b: tabs + (b*NXF + x)*R; set-independent
     // tables always use b = 0 (so a fused BC tile needs 3 slots, a plain A tile 1).  The two mbarriers sit between the
     // tile and the tables, at an address known at compile time (one register fewer to keep live across the tile loop).
-    uint64_t* bar = reinterpret_cast<uint64_t*>(smem + kTileChunks);
-    uint4* tabs = smem + kTileChunks + 1;
+    uint64_t* bar = reinterpret_cast<uint64_t*>(smem + kChunks);
+    uint4* tabs = smem + kChunks + 1;
     const bool var0 = P.xf[0].t1 != 0, var1 = NXF == 2 && P.xf[1].t1 != 0;
     const uint32_t tid  = threadIdx.x;
     const uint32_t groups = (P.nstrips + P.strips_per_item - 1) / P.strips_per_item;
     const uint32_t nitems = P.nsets * groups;
     constexpr uint32_t nsteps = NXF == 2 ? (LR > kStages ? 3u : 1u) : (LR > kStages ? 2u : 1u);
-    constexpr uint32_t kWt = 16384u >> LR;                // words per tile row
+    constexpr uint32_t kWt = (1u << Geom<NT>::logw) >> LR;   // words per tile row
     constexpr uint32_t kRowsBox = R < 256u ? R : 256u;    // TMA box: kRowsBox rows x kWt words
     constexpr uint32_t kBoxes = R / kRowsBox;
 
@@ -98,7 +102,7 @@ __global__ void __launch_bounds__(kThreads, 2) ntt_pass_kernel(const PassParams 
     if (!tile_decode(P, groups, nitems, 0, cur_set, cur_strip)) return;
     uint32_t tb = 0;                                      // table buffer used by the current tile
     uint32_t phase = 0;
-    uint64_t* rbar = bar + 1;                             // "all eight warps have pulled the last step's slots into registers"
+    uint64_t* rbar = bar + 1;                             // "every warp has pulled the last step's slots into registers"
 
     // request tile (set, strip) [+ the set's tables into buffer tbuf]
     auto request = [&](uint32_t set, uint32_t strip, bool with_tables, uint32_t tbuf) {
@@ -107,7 +111,7 @@ __global__ void __launch_bounds__(kThreads, 2) ntt_pass_kernel(const PassParams 
                 fence_proxy_async();                      // order our earlier generic-proxy accesses to the tile before the async-proxy writes
                 const bool first = with_tables && tbuf == 2u;         // prologue: also the set-independent tables
                 const uint32_t ld0 = with_tables && (var0 || first), ld1 = NXF == 2 && with_tables && (var1 || first);
-                mbar_expect_tx(bar, kTileBytes + (ld0 + ld1) * (R * 16u));
+                mbar_expect_tx(bar, Geom<NT>::bytes + (ld0 + ld1) * (R * 16u));
 #pragma unroll
                 for (uint32_t b = 0; b < kBoxes; ++b)
                     tma_load_3d(tile + b * (kRowsBox * (kWt / 4)), &tmap, bar, strip * kWt, b * kRowsBox, set);
@@ -117,19 +121,19 @@ __global__ void __launch_bounds__(kThreads, 2) ntt_pass_kernel(const PassParams 
                 if (ld1) bulk_load(tabs + ((var1 ? tbv : 0u) * NXF + 1) * R, tsrc + R, R * 16u, bar);
             }
         } else {
-            load_tile_cpasync(P, set, strip, tid, tile);
+            load_tile_cpasync<NT>(P, set, strip, tid, tile);
             if (with_tables) {
                 const bool first = tbuf == 2u;
                 const uint32_t tbv = first ? 0u : tbuf;
                 const uint4* tsrc = P.tables + (size_t)set * P.table_set_stride;
-                if (var0 || first) for (uint32_t i = tid; i < R; i += kThreads) copy16(tabs + ((var0 ? tbv : 0u) * NXF + 0) * R + i, tsrc + i);
-                if (NXF == 2 && (var1 || first)) for (uint32_t i = tid; i < R; i += kThreads) copy16(tabs + ((var1 ? tbv : 0u) * NXF + 1) * R + i, tsrc + R + i);
+                if (var0 || first) for (uint32_t i = tid; i < R; i += NT) copy16(tabs + ((var0 ? tbv : 0u) * NXF + 0) * R + i, tsrc + i);
+                if (NXF == 2 && (var1 || first)) for (uint32_t i = tid; i < R; i += NT) copy16(tabs + ((var1 ? tbv : 0u) * NXF + 1) * R + i, tsrc + R + i);
             }
         }
     };
 
     if (TMA) {
-        if (tid == 0) { mbar_init(bar, 1); mbar_init(rbar, kThreads / 32); fence_mbar_init(); }
+        if (tid == 0) { mbar_init(bar, 1); mbar_init(rbar, NT / 32); fence_mbar_init(); }
         __syncthreads();
     }
     request(cur_set, cur_strip, true, 2u);                // prologue: first tile + all its tables (buffer 0)
@@ -137,13 +141,13 @@ __global__ void __launch_bounds__(kThreads, 2) ntt_pass_kernel(const PassParams 
     for (uint32_t t = 0;; ++t) {
         if (TMA) mbar_wait(bar, phase);
         else     { cp_async_wait_all(); __syncthreads(); }
-        const bool active = thread_active(P, tid, cur_strip);
+        const bool active = thread_active<NT>(P, tid, cur_strip);
         RoundRegs r;
 #pragma unroll 1
         for (uint32_t s = 0; s < nsteps; ++s) {
             const Step st = step_of(LR, NXF, s);
             const bool last = s + 1 == nsteps;
-            if (active) round_read(P, st.k, st.xfi == 0, tid, tile, r);
+            if (active) round_read<NT>(P, st.k, st.xfi == 0, tid, tile, r);
             if (last) {                                   // every slot is in registers: the tile buffer is free.
                 if (TMA) {                                // each warp reports in; only the issuing thread waits for all of them
                     __syncwarp();
@@ -162,13 +166,13 @@ __global__ void __launch_bounds__(kThreads, 2) ntt_pass_kernel(const PassParams 
             const uint4* tw0 = tabs + ((var0 ? tb : 0u) * NXF) * R;
             const uint4* tw1 = tabs + ((var1 ? tb : 0u) * NXF + 1) * R;
             #if !defined(FECC_SKIP_MATH)                                   // -DFECC_SKIP_MATH: copy-only build for measuring the memory floor of a pass
-            if (active) round_math(P, st, tid, cur_set, tw0, tw1, r);
+            if (active) round_math<NT>(P, st, tid, cur_set, tw0, tw1, r);
 #endif
             if (!last) {
-                if (active) round_write_tile(P, st.k, st.xfi == 0, tid, tile, r);
+                if (active) round_write_tile<NT>(P, st.k, st.xfi == 0, tid, tile, r);
                 __syncthreads();
             } else if (active) {
-                round_write_global(P, st, tid, cur_set, cur_strip, r);
+                round_write_global<NT>(P, st, tid, cur_set, cur_strip, r);
             }
         }
         uint32_t nxt_set, nxt_strip;                      // (re)decoded here, where registers are plentiful
@@ -204,11 +208,11 @@ cudaError_t launch_build_tables(PassParams& P, uint4* out, cudaStream_t stream)
 
 // shared memory of the CTA-level kernel: tile + two mbarriers + table slots.  Table slot of transform x in buffer b is
 // (b*nxf + x); buffer 1 is needed only up to the last set-dependent transform.
-size_t pass_smem_bytes(const PassParams& P)
+size_t pass_smem_bytes(const PassParams& P, uint32_t tile_bytes)
 {
     uint32_t slots = P.nxf;                                            // buffer 0
     if (P.nxf == 2 && P.xf[1].t1) slots = 4; else if (P.xf[0].t1) slots = P.nxf + 1;
-    return (size_t)kTileBytes + (size_t)slots * ((size_t)16 << P.log_r) + 16;
+    return (size_t)tile_bytes + (size_t)slots * ((size_t)16 << P.log_r) + 16;
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -225,12 +229,13 @@ static EncodeTiledFn encode_tiled()
     return fn;
 }
 
-// 3-D view of the source buffer: [word][row within set][set]; box = one tile row strip of <= 256 rows.
-static bool make_tensor_map(const PassParams& P, CUtensorMap* map)
+// 3-D view of the source buffer: [word][row within set][set]; box = one tile row strip of <= 256 rows, of the tile's
+// row width (tile_words / R words).
+static bool make_tensor_map(const PassParams& P, uint32_t tile_words, CUtensorMap* map)
 {
     EncodeTiledFn enc = encode_tiled();
     if (!enc) return false;
-    const uint32_t R = 1u << P.log_r, Wt = 16384u >> P.log_r;
+    const uint32_t R = 1u << P.log_r, Wt = tile_words >> P.log_r;
     if (Wt > 256) return false;
     const cuuint64_t row_bytes = (cuuint64_t)P.pitch4 * 16;
     cuuint64_t gdim[3] = {(cuuint64_t)P.s4 * 4, R, P.nsets};
@@ -245,44 +250,56 @@ static bool make_tensor_map(const PassParams& P, CUtensorMap* map)
 template <int LR, int NXF, int TMA>
 static cudaError_t launch_inst(const PassParams& P, const CUtensorMap& map, unsigned grid, cudaStream_t stream)
 {
+    constexpr int NT = pass_threads(LR, NXF, TMA);
     static bool attr_set = false;
     if (!attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(ntt_pass_kernel<LR, NXF, TMA>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             kTileBytes + 2 * NXF * (16 << LR) + 16);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(ntt_pass_kernel<LR, NXF, TMA>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+        cudaError_t e = cudaFuncSetAttribute(ntt_pass_kernel<LR, NXF, TMA, NT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             Geom<NT>::bytes + 2 * NXF * (16 << LR) + 16);
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(ntt_pass_kernel<LR, NXF, TMA, NT>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
         if (e != cudaSuccess) return e;
         attr_set = true;
     }
-    ntt_pass_kernel<LR, NXF, TMA><<<grid, kThreads, pass_smem_bytes(P), stream>>>(P, map);
+    ntt_pass_kernel<LR, NXF, TMA, NT><<<grid, NT, pass_smem_bytes(P, Geom<NT>::bytes), stream>>>(P, map);
     return cudaGetLastError();
 }
 
-// name of the instantiation a pass is dispatched to, for the per-kernel lines of the benchmark (static storage)
-static const char* kernel_name(uint32_t lr, uint32_t nxf, uint32_t tma)
+// name of the instantiation a pass is dispatched to, for the per-kernel lines of the benchmark (static storage);
+// wide instantiations carry their thread count
+static const char* kernel_name(uint32_t lr, uint32_t nxf, uint32_t tma, int nt)
 {
     static char names[6][3][3][40];
     char* n = names[lr - 5][nxf][tma];
-    if (!n[0]) snprintf(n, 40, "ntt_pass_kernel<%u,%u,%u>", lr, nxf, tma);
+    if (!n[0]) {
+        if (nt == kThreads) snprintf(n, 40, "ntt_pass_kernel<%u,%u,%u>", lr, nxf, tma);
+        else                snprintf(n, 40, "ntt_pass_kernel<%u,%u,%u,%d>", lr, nxf, tma, nt);
+    }
     return n;
 }
 
+// The planner lays every pass out for the narrow geometry; the launcher picks the instantiation and, for a wide one,
+// re-lays the strips of its copy of the descriptor (the plans and their CPU emulation stay geometry-free).
 cudaError_t launch_pass(const PassParams& Pin, int num_sms, cudaStream_t stream, const char** kernel)
 {
     PassParams P = Pin;
+    if (!P.tables) return cudaErrorInvalidValue;
+    static const bool no_tma = getenv("FASTECC_B200_NO_TMA") != nullptr;
+    const uint32_t tmak = P.log_g ? 2u : 1u;
+    int nt = !no_tma && P.log_r >= 6 ? pass_threads((int)P.log_r, (int)P.nxf, (int)tmak) : kThreads;
+    if (nt == kWideThreads) set_strips<kWideThreads>(P);
+    CUtensorMap map;
+    memset(&map, 0, sizeof map);
+    const bool tma = !no_tma && P.log_r >= 6 && make_tensor_map(P, nt == kWideThreads ? 1u << Geom<kWideThreads>::logw : 1u << Geom<kThreads>::logw, &map);
+    if (!tma && nt != kThreads) { P = Pin; nt = kThreads; }     // the wide instantiations load by TMA only
+    if (P.log_g && !tma) return cudaErrorNotSupported;          // sharded stores exist only in the TMA instantiations
+
     const uint32_t groups = (P.nstrips + P.strips_per_item - 1) / P.strips_per_item;
     const unsigned long long nitems = (unsigned long long)P.nsets * groups;
-    static const int ctas_per_sm = getenv("FASTECC_B200_CTAS_PER_SM") ? atoi(getenv("FASTECC_B200_CTAS_PER_SM")) : 2;   // tuning knob
-    unsigned long long grid = (unsigned long long)num_sms * (ctas_per_sm > 0 ? ctas_per_sm : 2);
+    static const int ctas_per_sm = getenv("FASTECC_B200_CTAS_PER_SM") ? atoi(getenv("FASTECC_B200_CTAS_PER_SM")) : 2;   // narrow kernels
+    unsigned long long grid = (unsigned long long)num_sms * (nt == kWideThreads ? 1 : ctas_per_sm > 0 ? ctas_per_sm : 2);
     if (grid > nitems) grid = nitems;
     if (grid == 0) return cudaSuccess;
     const unsigned g = (unsigned)grid;
-    if (!P.tables) return cudaErrorInvalidValue;
-    CUtensorMap map;
-    memset(&map, 0, sizeof map);
-    static const bool no_tma = getenv("FASTECC_B200_NO_TMA") != nullptr;
-    const bool tma = !no_tma && P.log_r >= 6 && make_tensor_map(P, &map);
-    if (P.log_g && !tma) return cudaErrorNotSupported;          // sharded stores exist only in the TMA instantiations
-    if (kernel) *kernel = kernel_name(P.log_r, P.nxf, tma ? (P.log_g ? 2 : 1) : 0);
+    if (kernel) *kernel = kernel_name(P.log_r, P.nxf, tma ? tmak : 0, nt);
 #define FECC_CASE(L) case L: \
         if (tma && P.log_g) return P.nxf == 2 ? launch_inst<L, 2, 2>(P, map, g, stream) : launch_inst<L, 1, 2>(P, map, g, stream); \
         if (tma) return P.nxf == 2 ? launch_inst<L, 2, 1>(P, map, g, stream) : launch_inst<L, 1, 1>(P, map, g, stream); \

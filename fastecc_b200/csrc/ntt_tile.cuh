@@ -1,4 +1,4 @@
-// Tile-level decimation-in-time NTT over GF(0xFFF00001): the code every pass kernel runs per 64 KiB tile.
+// Tile-level decimation-in-time NTT over GF(0xFFF00001): the code every pass kernel runs per 64 or 128 KiB tile.
 //
 // This header is the GPU counterpart of the reference's inner loops
 //     IterativeNTT_Steps  ntt.cpp:251-284   (radix-2 butterflies across blocks, inner loop over the SIZE words)
@@ -9,10 +9,11 @@
 // index/twiddle logic can be executed thread-by-thread on the CPU (tests/emulate_tile.cu) before it ever
 // touches a GPU.
 //
-// Geometry.  A tile is R = 2^LR rows (blocks) x WT words, R*WT = 16384 words (64 KiB of shared memory), stored as
-// 16-byte chunks: chunk (row p, q) at index p*(WT/4)+q.  256 threads; thread (j, q2) owns the word PAIR q2 of every
-// row it touches (the word dimension is a pure batch dimension, SURVEY 7 "hard part 2") and, in every round,
-// 32 rows: q2 = tid % (WT/2), j = tid / (WT/2) in [0, R/32).  Thirty-two rows x two words = 64 data registers.
+// Geometry.  A tile is R = 2^LR rows (blocks) x WT words, R*WT = 16384 words (64 KiB of shared memory, 256 threads) or
+// 32768 words (128 KiB, 512 threads: the wide geometry, Geom<512>), stored as 16-byte chunks: chunk (row p, q) at index
+// p*(WT/4)+q.  Thread (j, q2) owns the word PAIR q2 of every row it touches (the word dimension is a pure batch
+// dimension, SURVEY 7 "hard part 2") and, in every round, 32 rows: q2 = tid % (WT/2), j = tid / (WT/2) in [0, R/32).
+// Thirty-two rows x two words = 64 data registers in either geometry; only the (j, q2) mapping differs.
 //
 // Rounds.  A size-R DIT transform runs ceil(LR/5) <= 2 rounds.  Round 0 holds index bits [0,5) in-thread and
 // executes the stages of bits [0, min(5,LR)); round 1 holds bits [LR-5, LR) and executes the stages of bits
@@ -49,13 +50,36 @@
 
 namespace fecc {
 
-constexpr int kThreads    = 256;
-constexpr int kTileChunks = 4096;            // 16-byte chunks per tile
+constexpr int kThreads    = 256;             // the narrow (default) geometry: threads per CTA ...
+constexpr int kTileChunks = 4096;            // ... and 16-byte chunks per tile
 constexpr int kTileBytes  = kTileChunks * 16;
+constexpr int kWideThreads = 512;            // the wide geometry: one CTA per SM over a 128 KiB tile
 constexpr int kMaxLogR    = 10;
 constexpr int kMinLogR    = 5;
 constexpr int kRows       = 32;              // rows held by a thread in a round
 constexpr int kStages     = 5;               // radix-2 stages per full round
+
+// Geometry of a CTA: NT threads, each holding 32 rows x one word pair = 16 chunks, so a tile is 16*NT chunks of 2^LOGW
+// words.  NT = 256: 64 KiB tiles, rows of 2^(14-LR) words.  NT = 512: 128 KiB tiles, rows of 2^(15-LR) words (128-byte
+// rows at LR = 10).  Every index function below takes NT as a template parameter defaulting to the narrow geometry.
+template <int NT> struct Geom {
+    static constexpr int      threads = NT;
+    static constexpr int      chunks  = 16 * NT;
+    static constexpr uint32_t bytes   = 16u * chunks;
+    static constexpr uint32_t logw    = NT == 512 ? 15 : NT == 256 ? 14 : 0;    // log2(words per tile)
+    static_assert(logw != 0, "tile geometries: 256 or 512 threads");
+};
+
+// Geometry of the pass-kernel instantiation <LR, NXF, TMA> (ntt_pass.cu; the CPU emulation asks the same question).  The fused
+// 1024-row pass runs wide: its narrow tile has 64-byte rows (2-way bank conflicts, 64-byte DRAM pieces, two copies of the stage
+// tables per SM).  -DFECC_WIDE_A (A/B build only) runs the 512-row single-transform pass wide as well.
+#if !defined(FECC_WIDE_A)
+#define FECC_WIDE_A 0
+#endif
+FECC_HD constexpr int pass_threads(int LR, int NXF, int TMA)
+{
+    return TMA == 1 && ((LR == 10 && NXF == 2) || (FECC_WIDE_A && LR == 9 && NXF == 1)) ? kWideThreads : kThreads;
+}
 
 struct Xform { uint32_t z, t0, t1; };        // tile root g^z; input twist g^(t0 + set*t1)   (exponents mod 2^20)
 
@@ -175,9 +199,10 @@ FECC_HD void bfly2_trivial(uint2& a, uint2& b)
 }
 
 struct ThreadPos { uint32_t q2, j, q2log; };
+template <int NT = kThreads>
 FECC_HD ThreadPos thread_pos(uint32_t LR, uint32_t tid)
 {
-    ThreadPos t; t.q2log = 13 - LR; t.q2 = tid & ((1u << t.q2log) - 1u); t.j = tid >> t.q2log; return t;
+    ThreadPos t; t.q2log = Geom<NT>::logw - 1 - LR; t.q2 = tid & ((1u << t.q2log) - 1u); t.j = tid >> t.q2log; return t;
 }
 
 // Slot bookkeeping of one thread in one round.
@@ -300,8 +325,8 @@ FECC_HD Xform get_xf(const PassParams& P, uint32_t xfi)
 
 // ---------------------------------------------------------------------------------------------------------------
 // Per-thread steps of a tile.  The kernel (ntt_pass.cu) runs them with block barriers in between; the CPU
-// emulation (tests/emulate_tile.cu) runs each step for tid = 0..255 in turn, which is equivalent because within a
-// step a thread only touches its own slots.
+// emulation (tests/emulate_tile.cu, tests/emulate_wide.cu) runs each step for tid = 0..NT-1 in turn, which is
+// equivalent because within a step a thread only touches its own slots.
 // ---------------------------------------------------------------------------------------------------------------
 namespace fecc {
 
@@ -325,44 +350,61 @@ FECC_HD uint32_t table_entry_exponent(const PassParams& P, uint32_t xfi, uint32_
 }
 
 // 16-byte cp.async fallback loader (LR == 5, or FASTECC_B200_NO_TMA=1): tile row p <- source row p of the set,
-// natural order.  Thread tid moves chunks c = tid + 256*m.
+// natural order.  Thread tid moves chunks c = tid + NT*m.
+template <int NT = kThreads>
 FECC_HD void load_tile_cpasync(const PassParams& P, uint32_t set, uint32_t strip, uint32_t tid, uint4* tile)
 {
-    const uint32_t LR = P.log_r, qlog = 12 - LR, Q = 1u << qlog;
+    const uint32_t LR = P.log_r, qlog = Geom<NT>::logw - 2 - LR, Q = 1u << qlog;
     const uint32_t p0 = tid >> qlog, qq = tid & (Q - 1);
     const uint32_t gcol = strip * Q + qq;
-    const uint32_t prow = (uint32_t)kThreads >> qlog;                 // tile rows covered by one sweep of the CTA
+    const uint32_t prow = (uint32_t)NT >> qlog;                       // tile rows covered by one sweep of the CTA
     if (gcol >= P.s4) {                                               // beyond the row: keep the tile defined (TMA zero-fills)
 #pragma unroll
-        for (int m = 0; m < 16; ++m) tile[tid + (uint32_t)kThreads * m] = make_uint4(0, 0, 0, 0);
+        for (int m = 0; m < 16; ++m) tile[tid + (uint32_t)NT * m] = make_uint4(0, 0, 0, 0);
         return;
     }
     const uint32_t row0 = set * P.src_set_stride + p0 * P.src_row_stride;
     const uint4* g = reinterpret_cast<const uint4*>(P.src) + ((size_t)row0 * P.pitch4 + gcol);
     const size_t gstep = (size_t)prow * P.src_row_stride * P.pitch4;
 #pragma unroll
-    for (int m = 0; m < 16; ++m) { copy16(tile + tid + (uint32_t)kThreads * m, g); g += gstep; }
+    for (int m = 0; m < 16; ++m) { copy16(tile + tid + (uint32_t)NT * m, g); g += gstep; }
 }
 // ... and the set's precomputed stage tables (a contiguous nxf*R*16-byte block)
+template <int NT = kThreads>
 FECC_HD void load_tables_cpasync(const PassParams& P, uint32_t set, uint32_t tid, uint4* tabs)
 {
     const uint32_t n = P.nxf << P.log_r;
     const uint4* src = P.tables + (size_t)set * P.table_set_stride;
-    for (uint32_t i = tid; i < n; i += kThreads) copy16(tabs + i, src + i);
+    for (uint32_t i = tid; i < n; i += NT) copy16(tabs + i, src + i);
 }
 
+// word pairs per tile row (the column width of a strip)
+template <int NT = kThreads>
+FECC_HD uint32_t strip_pairs(uint32_t LR) { return (1u << (Geom<NT>::logw - 1)) >> LR; }
+
+template <int NT = kThreads>
 FECC_HD bool thread_active(const PassParams& P, uint32_t tid, uint32_t strip)
 {
-    const ThreadPos tp = thread_pos(P.log_r, tid);
-    const uint32_t words2 = strip * (8192u >> P.log_r) + tp.q2;     // word-pair column inside the row
-    return (words2 >> 1) < P.s4;                                    // partial last strip: beyond the row's last chunk
+    const ThreadPos tp = thread_pos<NT>(P.log_r, tid);
+    const uint32_t words2 = strip * strip_pairs<NT>(P.log_r) + tp.q2;     // word-pair column inside the row
+    return (words2 >> 1) < P.s4;                                          // partial last strip: beyond the row's last chunk
+}
+
+// The strip layout of a pass in geometry NT, the one copy of the rule (plan.h's base_pass() lays passes out for the narrow
+// geometry; the launcher re-lays a pass it runs wide): strips of the tile's row width, and 4 consecutive strips of a set per
+// work item where that divides evenly (table reuse; tile_decode in ntt_pass.cu needs strips_per_item to divide nstrips).
+template <int NT>
+FECC_HD void set_strips(PassParams& P)
+{
+    const uint32_t Q = (uint32_t)Geom<NT>::chunks >> P.log_r;       // 16-byte chunks per tile row
+    P.nstrips = (P.s4 + Q - 1) / Q;
+    P.strips_per_item = (P.nstrips >= 16 && P.nstrips % 4 == 0) ? 4 : 1;
 }
 
 // Tile address (in uint2 units) of the thread's slot i in round c:  physical row = bitrev(slot) for the first
 // transform of a tile (brev), = slot for the second.  Both reduce to "base + i*step" with compile-time i.
-// (Tiles of 1024 rows have 64-byte rows and every shared-memory access of theirs is a 2-way bank conflict; the
-// parity row swap that removes the conflicts was measured and is NOT used: it needs a block barrier between the first
-// read and the first write of a tile, and the fused pass got 5 % slower with it -- DESIGN.md section 12.)
+// (Narrow tiles of 1024 rows have 64-byte rows and three of their four access patterns are 2-way bank conflicted; the
+// wide geometry gives the same rows 128 bytes and is conflict-free, tools/banksim_cta.py.  The fused pass runs wide.)
 #define FECC_SLOT_LOOP(ACCESS)                                                                                     \
     if (brev) {                                                                                                    \
         uint32_t a = (bitrev(c.jbase, LR) << tp.q2log) | tp.q2;                                                    \
@@ -375,10 +417,11 @@ FECC_HD bool thread_active(const PassParams& P, uint32_t tid, uint32_t strip)
     }
 
 // (a) read the thread's 32 slots of a step.  brev = bit-reversed placement (every round of the FIRST transform).
+template <int NT = kThreads>
 FECC_HD void round_read(const PassParams& P, uint32_t k, uint32_t brev, uint32_t tid, const uint4* tile, RoundRegs& r)
 {
     const uint32_t LR = P.log_r;
-    const ThreadPos tp = thread_pos(LR, tid);
+    const ThreadPos tp = thread_pos<NT>(LR, tid);
     const RoundCtx c = make_round(LR, k, tp.j);
     const uint2* t2 = reinterpret_cast<const uint2*>(tile);
 #define FECC_RD(I, A) r.x[I] = t2[A]
@@ -387,10 +430,11 @@ FECC_HD void round_read(const PassParams& P, uint32_t k, uint32_t brev, uint32_t
 }
 
 // (b) the butterflies of a step
+template <int NT = kThreads>
 FECC_HD void round_math(const PassParams& P, const Step st, uint32_t tid, uint32_t set, const uint4* tw0, const uint4* tw1, RoundRegs& r)
 {
     const uint32_t LR = P.log_r;
-    const ThreadPos tp = thread_pos(LR, tid);
+    const ThreadPos tp = thread_pos<NT>(LR, tid);
     const RoundCtx c = make_round(LR, st.k, tp.j);
     const bool first = (st.xfi == 0 && st.k == 0);
     const Xform xf = get_xf(P, st.xfi);
@@ -413,10 +457,11 @@ FECC_HD void round_math(const PassParams& P, const Step st, uint32_t tid, uint32
 }
 
 // (c) write back in place ...
+template <int NT = kThreads>
 FECC_HD void round_write_tile(const PassParams& P, uint32_t k, uint32_t brev, uint32_t tid, uint4* tile, const RoundRegs& r)
 {
     const uint32_t LR = P.log_r;
-    const ThreadPos tp = thread_pos(LR, tid);
+    const ThreadPos tp = thread_pos<NT>(LR, tid);
     const RoundCtx c = make_round(LR, k, tp.j);
     uint2* t2 = reinterpret_cast<uint2*>(tile);
 #define FECC_WR(I, A) t2[A] = r.x[I]
@@ -444,13 +489,14 @@ FECC_HD void store_global2(uint2* p, uint2 v)
     *p = v;
 #endif
 }
+template <int NT = kThreads>
 FECC_HD void round_write_global(const PassParams& P, const Step st, uint32_t tid, uint32_t set, uint32_t strip, RoundRegs& r)
 {
-    const ThreadPos tp = thread_pos(P.log_r, tid);
+    const ThreadPos tp = thread_pos<NT>(P.log_r, tid);
     // the last step is the fused one only when a fused tile has a single round (LR <= 5): compile-time in the kernel
     const bool fused_last = (P.nxf == 2) && (num_rounds(P.log_r) == 1);
     const RoundCtx c = fused_last ? make_round(P.log_r, 0, 0) : make_round(P.log_r, st.k, tp.j);
-    const uint32_t gcol2 = strip * (8192u >> P.log_r) + tp.q2;
+    const uint32_t gcol2 = strip * strip_pairs<NT>(P.log_r) + tp.q2;
     // sharded, exchange fused into the stores: this thread's output elements jbase + (i << lb) all have the same residue
     // mod G (plan.h guarantees lb >= log_g), i.e. one destination GPU per thread, chosen here once per tile
     uint32_t* base = P.dst;

@@ -32,9 +32,12 @@ namespace fecc {
 inline uint32_t ilog2(size_t n) { uint32_t l = 0; while (((size_t)1 << l) < n) ++l; return l; }
 inline bool     is_pow2(size_t n) { return n && !(n & (n - 1)); }
 // N = N1*N2: log2 of the factor handled by the strided passes (A, D; A').  Strided passes touch a different DRAM page
-// per row, so they want wide rows: a 512-row tile has 128-byte rows (measured memory floor 0.94 ms per pass at the
-// headline size) where a 1024-row tile has 64-byte rows (1.40 ms).  Hence L1 <= 9 whenever N2 = N/N1 still fits a
-// tile (<= 1024): 2^19 = 512 x 1024, with the longer, contiguous-row work in the fused pass.
+// per row, so they want wide rows.  Copy-only floors at the headline size on an H100 SXM at a 400 W limit (-DFECC_SKIP_MATH,
+// DESIGN.md section 6): a 512-row tile with 128-byte rows 1.68 ms per pass; the fused pass's 1024-row tile with 64-byte rows
+// (256 threads) 3.15 ms, in the 512-thread geometry it runs in (128-byte rows, no bank conflicts, one CTA per SM) 1.58 ms.
+// (Those floors include every shared-memory round: they measure the geometry as a whole, not DRAM granularity alone.)  So the
+// fused pass's rows are made wide by its geometry, not by the split: L1 <= 9 whenever N2 = N/N1 still fits a tile (<= 1024):
+// 2^19 = 512 x 1024, with the longer work in the fused pass.
 // FASTECC_B200_SPLIT=hi|lo overrides (ceil / floor of LN/2) for experiments.
 inline uint32_t split_l1(uint32_t LN)
 {
@@ -62,9 +65,7 @@ inline PassParams base_pass(const Buffers& b, uint32_t log_r)
     p.pitch4 = b.pitch_words / 4;
     p.s4 = (b.size_words + 3) / 4;
     p.log_r = log_r;
-    const uint32_t Q = 4096u >> log_r;                                  // 16-byte chunks per tile row
-    p.nstrips = (p.s4 + Q - 1) / Q;
-    p.strips_per_item = (p.nstrips >= 16 && p.nstrips % 4 == 0) ? 4 : 1;   // must divide nstrips (ntt_pass.cu tile_decode)
+    set_strips<kThreads>(p);                                            // narrow layout; launch_pass re-lays a pass it runs wide
     p.nxf = 1;
     return p;
 }
