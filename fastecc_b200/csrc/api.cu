@@ -531,7 +531,7 @@ int fastecc_b200_rs_encode_dev_timed(uint32_t* d, size_t N, size_t size, size_t 
 int fastecc_b200_shard_geometry(size_t N, int n_ranks, size_t* N1, size_t* N2, int* fused_exchange_ok)
 {
     if (!is_pow2(N) || N < 2) return fail(FASTECC_B200_EINVAL, "fastecc_b200_shard_geometry: N must be a power of two");
-    const uint32_t LN = ilog2(N), L1 = LN <= (uint32_t)kMaxLogR ? LN : split_l1(LN);
+    const uint32_t LN = ilog2(N), L1 = LN <= (uint32_t)kMaxLogR ? LN : split_l1(LN, true);
     if (N1) *N1 = (size_t)1 << L1;
     if (N2) *N2 = (size_t)1 << (LN - L1);
     if (fused_exchange_ok) *fused_exchange_ok = n_ranks >= 2 ? (shard_p2p_supported(N, (uint32_t)n_ranks) ? 1 : 0) | (ntt_shard_p2p_supported(N, (uint32_t)n_ranks) ? 2 : 0) : 0;

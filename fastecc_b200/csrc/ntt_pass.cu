@@ -3,8 +3,8 @@
 // the RS scaling (RS.cpp:51-59) and the start of the forward transform in a single pass.
 //
 // Execution model (DESIGN.md section 5): persistent CTAs of 256 threads, two per SM, each walking a sequence of
-// 64 KiB tiles (row set x column strip); the fused 1024-row pass instead runs one CTA of 512 threads per SM over 128 KiB
-// tiles with 128-byte rows (pass_threads() in ntt_tile.cuh).  Per tile:
+// 64 KiB tiles (row set x column strip); the 1024-row passes and the fused 512-row pass instead run one CTA of 512 threads
+// per SM over 128 KiB tiles with rows of at least 128 bytes (pass_threads() in ntt_tile.cuh).  Per tile:
 //   * one elected thread issues the TMA traffic: cp.async.bulk.tensor (3-D tensor map over [word][row-in-set][set],
 //     boxes of <= 256 rows) for the tile and, when the row set changes, one cp.async.bulk for the set's precomputed
 //     twiddle tables; completion is tracked by an mbarrier (expect_tx / complete_tx).  The next tile is requested
@@ -143,10 +143,9 @@ __global__ void __launch_bounds__(NT, NT == kWideThreads ? 1 : 2) ntt_pass_kerne
         else     { cp_async_wait_all(); __syncthreads(); }
         const bool active = thread_active<NT>(P, tid, cur_strip);
         RoundRegs r;
-        // The wide fused pass (BC of the headline encode) unrolls its three steps: every round's slot offsets, table strides and
-        // stage ranges become immediates, and BC runs about 7 % faster at the same 128 registers without spills (DESIGN.md
-        // section 6).  The other instantiations keep one copy of the step body: unrolled, several of them spill.
-#pragma unroll (NT == kWideThreads ? nsteps : 1)
+        // pass_unrolled() (ntt_tile.cuh): the wide passes unroll their steps, at the same 128 registers without spills; the
+        // fused ones run about 7 % faster so, the single-transform one about 4 % (DESIGN.md section 6).
+#pragma unroll (pass_unrolled(LR, NXF, TMA) ? nsteps : 1)
         for (uint32_t s = 0; s < nsteps; ++s) {
             const Step st = step_of(LR, NXF, s);
             const bool last = s + 1 == nsteps;
@@ -250,10 +249,9 @@ static bool make_tensor_map(const PassParams& P, uint32_t tile_words, CUtensorMa
                CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-template <int LR, int NXF, int TMA>
+template <int LR, int NXF, int TMA, int NT = pass_threads(LR, NXF, TMA)>
 static cudaError_t launch_inst(const PassParams& P, const CUtensorMap& map, unsigned grid, cudaStream_t stream)
 {
-    constexpr int NT = pass_threads(LR, NXF, TMA);
     static bool attr_set = false;
     if (!attr_set) {
         cudaError_t e = cudaFuncSetAttribute(ntt_pass_kernel<LR, NXF, TMA, NT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -264,6 +262,15 @@ static cudaError_t launch_inst(const PassParams& P, const CUtensorMap& map, unsi
     }
     ntt_pass_kernel<LR, NXF, TMA, NT><<<grid, NT, pass_smem_bytes(P, Geom<NT>::bytes), stream>>>(P, map);
     return cudaGetLastError();
+}
+
+// the TMA instantiation of a single-GPU pass in geometry nt (the narrow twin where pass_has_narrow_twin)
+template <int LR, int NXF>
+static cudaError_t launch_tma(const PassParams& P, const CUtensorMap& map, unsigned grid, cudaStream_t stream, int nt)
+{
+    if constexpr (pass_has_narrow_twin(LR, NXF, 1))
+        if (nt == kThreads) return launch_inst<LR, NXF, 1, kThreads>(P, map, grid, stream);
+    return launch_inst<LR, NXF, 1>(P, map, grid, stream);
 }
 
 // name of the instantiation a pass is dispatched to, for the per-kernel lines of the benchmark (static storage);
@@ -289,6 +296,9 @@ cudaError_t launch_pass(const PassParams& Pin, int num_sms, cudaStream_t stream,
     const uint32_t tmak = P.log_g ? 2u : 1u;
     int nt = !no_tma && P.log_r >= 6 ? pass_threads((int)P.log_r, (int)P.nxf, (int)tmak) : kThreads;
     if (nt == kWideThreads) set_strips<kWideThreads>(P);
+    if (nt == kWideThreads && pass_has_narrow_twin((int)P.log_r, (int)P.nxf, (int)tmak) && (unsigned long long)P.nsets * P.nstrips < (unsigned)num_sms) {
+        P = Pin; nt = kThreads;                                 // fewer wide tiles than SMs: the narrow twin has twice as many
+    }
     CUtensorMap map;
     memset(&map, 0, sizeof map);
     const bool tma = !no_tma && P.log_r >= 6 && make_tensor_map(P, nt == kWideThreads ? 1u << Geom<kWideThreads>::logw : 1u << Geom<kThreads>::logw, &map);
@@ -305,7 +315,7 @@ cudaError_t launch_pass(const PassParams& Pin, int num_sms, cudaStream_t stream,
     if (kernel) *kernel = kernel_name(P.log_r, P.nxf, tma ? tmak : 0, nt);
 #define FECC_CASE(L) case L: \
         if (tma && P.log_g) return P.nxf == 2 ? launch_inst<L, 2, 2>(P, map, g, stream) : launch_inst<L, 1, 2>(P, map, g, stream); \
-        if (tma) return P.nxf == 2 ? launch_inst<L, 2, 1>(P, map, g, stream) : launch_inst<L, 1, 1>(P, map, g, stream); \
+        if (tma) return P.nxf == 2 ? launch_tma<L, 2>(P, map, g, stream, nt) : launch_tma<L, 1>(P, map, g, stream, nt); \
         else     return P.nxf == 2 ? launch_inst<L, 2, 0>(P, map, g, stream) : launch_inst<L, 1, 0>(P, map, g, stream);
     switch (P.log_r) {
         FECC_CASE(5) FECC_CASE(6) FECC_CASE(7) FECC_CASE(8) FECC_CASE(9) FECC_CASE(10)

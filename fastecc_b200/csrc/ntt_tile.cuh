@@ -70,15 +70,32 @@ template <int NT> struct Geom {
     static_assert(logw != 0, "tile geometries: 256 or 512 threads");
 };
 
-// Geometry of the pass-kernel instantiation <LR, NXF, TMA> (ntt_pass.cu; the CPU emulation asks the same question).  The fused
-// 1024-row pass runs wide: its narrow tile has 64-byte rows (2-way bank conflicts, 64-byte DRAM pieces, two copies of the stage
-// tables per SM).  -DFECC_WIDE_A (A/B build only) runs the 512-row single-transform pass wide as well.
+// Geometry of the pass-kernel instantiation <LR, NXF, TMA> (ntt_pass.cu; the CPU emulation asks the same question).  Wide: the
+// 1024-row passes, fused or single-transform, whose narrow tile has 64-byte rows (2-way bank conflicts, 64-byte DRAM pieces, two
+// copies of the stage tables per SM), and the 512-row fused pass (BC of the 2^18 and 2^19 encodes), which runs its butterflies
+// about 7 % faster wide with its steps unrolled (DESIGN.md section 6).  The sharded instantiations (TMA == 2) stay narrow.
+// -DFECC_WIDE_A (A/B build only) runs the 512-row single-transform pass wide as well.
 #if !defined(FECC_WIDE_A)
 #define FECC_WIDE_A 0
 #endif
 FECC_HD constexpr int pass_threads(int LR, int NXF, int TMA)
 {
-    return TMA == 1 && ((LR == 10 && NXF == 2) || (FECC_WIDE_A && LR == 9 && NXF == 1)) ? kWideThreads : kThreads;
+    return TMA == 1 && (LR == 10 || (LR == 9 && (NXF == 2 || FECC_WIDE_A))) ? kWideThreads : kThreads;
+}
+// Whether the instantiation unrolls its steps (ntt_pass.cu): every round's slot offsets, table strides and stage ranges then
+// become immediates.  The wide instantiations do, without spills at 128 registers.  The narrow ones keep one copy of the step
+// body: several spill unrolled, and <9,2,1> narrow, which did not, ran the 2^19 fused pass about 20 % slower unrolled (two CTAs
+// per SM in different parts of the longer code; DESIGN.md section 6).
+FECC_HD constexpr bool pass_unrolled(int LR, int NXF, int TMA)
+{
+    return pass_threads(LR, NXF, TMA) == kWideThreads;
+}
+// Whether the wide instantiation also has a narrow twin, which launch_pass (ntt_pass.cu) takes for a pass with fewer wide tiles
+// than SMs: the single-pass encode of 2^9 blocks (one row set) would otherwise leave most SMs idle with half as many tiles.  The
+// twin unrolls its steps like its wide sibling (pass_unrolled is per <LR, NXF, TMA>); with one tile per CTA that is faster.
+FECC_HD constexpr bool pass_has_narrow_twin(int LR, int NXF, int TMA)
+{
+    return pass_threads(LR, NXF, TMA) == kWideThreads && LR == 9 && NXF == 2;
 }
 
 struct Xform { uint32_t z, t0, t1; };        // tile root g^z; input twist g^(t0 + set*t1)   (exponents mod 2^20)

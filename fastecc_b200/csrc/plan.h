@@ -35,16 +35,26 @@ inline bool     is_pow2(size_t n) { return n && !(n & (n - 1)); }
 // per row, so they want wide rows.  Copy-only floors at the headline size on an H100 SXM at a 400 W limit (-DFECC_SKIP_MATH,
 // DESIGN.md section 6): a 512-row tile with 128-byte rows 1.68 ms per pass; the fused pass's 1024-row tile with 64-byte rows
 // (256 threads) 3.15 ms, in the 512-thread geometry it runs in (128-byte rows, no bank conflicts, one CTA per SM) 1.58 ms.
-// (Those floors include every shared-memory round: they measure the geometry as a whole, not DRAM granularity alone.)  So the
-// fused pass's rows are made wide by its geometry, not by the split: L1 <= 9 whenever N2 = N/N1 still fits a tile (<= 1024):
-// 2^19 = 512 x 1024, with the longer work in the fused pass.
-// FASTECC_B200_SPLIT=hi|lo overrides (ceil / floor of LN/2) for experiments.
-inline uint32_t split_l1(uint32_t LN)
+// (Those floors include every shared-memory round: they measure the geometry as a whole, not DRAM granularity alone.)  So rows
+// are made wide by the geometry, not by the split: every 1024-row pass and the fused 512-row pass run wide (pass_threads() in
+// ntt_tile.cuh).
+//   Single-GPU plans (plan_ntt, plan_encode, plan_encode_asym and the power-of-two transforms of the mixed-radix paths):
+//     L1 = ceil(LN/2), so the strided passes take the longer factor: 2^19 = 1024 x 512.  The fused pass BC, bound by its
+//     butterflies, then does 9 + 9 stages instead of 10 + 10, and A and D, bound by memory, one stage more each: the 2^19 encode
+//     runs about 2 % faster than with 512 x 1024 (DESIGN.md section 6).  Only 2^19 changes: 2^20 is 1024 x 1024 either way, and
+//     at 2^18 and below ceil(LN/2) <= 9.
+//   short_n1 = true: L1 <= 9 whenever N2 = N/N1 still fits a tile (<= 1024), so 2^19 = 512 x 1024.  For the sharded plans
+//     (shard_supported, plan_encode_shard[_p2p], shard_p2p_supported, ntt_shard_p2p_supported, plan_ntt_shard_p2p,
+//     fastecc_b200_shard_geometry): their instantiations are narrow (TMA == 2), where a 1024-row tile has 64-byte rows and
+//     64-byte remote stores.  And for the asymmetric encode to fewer parity blocks than the single-GPU N1 (asym_short_n1),
+//     which needs M >= N1.
+// FASTECC_B200_SPLIT=hi|lo overrides (ceil / floor of LN/2) for experiments; "lo" is the 512 x 1024 plan at 2^19 on one GPU.
+inline uint32_t split_l1(uint32_t LN, bool short_n1 = false)
 {
     static const char* env = getenv("FASTECC_B200_SPLIT");
     uint32_t L1 = (LN + 1) / 2;
     if (env && !strcmp(env, "lo")) L1 = LN / 2;
-    else if (!(env && !strcmp(env, "hi")) && L1 > 9) L1 = 9;
+    else if (!(env && !strcmp(env, "hi")) && short_n1 && L1 > 9) L1 = 9;
     if (L1 < (uint32_t)kMinLogR) L1 = kMinLogR;
     if (LN - L1 > (uint32_t)kMaxLogR) L1 = LN - kMaxLogR;
     return L1;
@@ -112,8 +122,8 @@ inline std::vector<PassParams> plan_ntt(const Buffers& b, size_t N, bool inverse
     return v;
 }
 
-// RS.cpp:41-63 on N data blocks -> N parity blocks, in place in b.x.
-inline std::vector<PassParams> plan_encode(const Buffers& b, size_t N)
+// RS.cpp:41-63 on N data blocks -> N parity blocks, in place in b.x.  short_n1: see split_l1.
+inline std::vector<PassParams> plan_encode(const Buffers& b, size_t N, bool short_n1 = false)
 {
     std::vector<PassParams> v;
     const uint32_t LN = ilog2(N);
@@ -131,7 +141,7 @@ inline std::vector<PassParams> plan_encode(const Buffers& b, size_t N)
         v.push_back(a);
         return v;
     }
-    const uint32_t L1 = split_l1(LN), L2 = LN - L1;
+    const uint32_t L1 = split_l1(LN, short_n1), L2 = LN - L1;
     const uint32_t N1 = 1u << L1, N2 = 1u << L2;
     PassParams a = base_pass(b, L1);
     a.src = b.x; a.dst = b.x; a.nsets = (uint32_t)N2;
@@ -160,18 +170,21 @@ inline std::vector<PassParams> plan_encode(const Buffers& b, size_t N)
 // the row sets j2 = 2^k * j2' of pass D: D runs on N2 / 2^k sets only and writes its result compactly (row j1*N2' + j2').
 // A is unchanged; BC writes to the scratch buffer b.y because D now reads rows that its compact output would overwrite.
 // Needs the two-level decomposition and M >= N1 (every wanted output still has j2 as its low digit); smaller M and
-// N <= 1024 are served by the caller from the smallest supported M (api.cu).  The first transform and the C half of BC
-// are not shortened yet (folding the coefficients before C needs the scaling as an explicit product first).
+// N <= 1024 are served by the caller from the smallest supported M (api.cu).  An M below the single-GPU N1 takes the short
+// split (2^19 = 512 x 1024), so M = 512 at 2^19 stays native.  The first transform and the C half of BC are not shortened yet
+// (folding the coefficients before C needs the scaling as an explicit product first).
+inline bool asym_short_n1(size_t N, size_t M) { return M < ((size_t)1 << split_l1(ilog2(N))); }
 inline bool asym_native(size_t N, size_t M)
 {
     const uint32_t LN = ilog2(N);
     if (LN <= (uint32_t)kMaxLogR || M >= N) return false;
-    return M >= ((size_t)1 << split_l1(LN));
+    return M >= ((size_t)1 << split_l1(LN, asym_short_n1(N, M)));
 }
 inline std::vector<PassParams> plan_encode_asym(const Buffers& b, size_t N, size_t M)
 {
-    std::vector<PassParams> v = plan_encode(b, N);                     // A, BC, D
-    const uint32_t LN = ilog2(N), L1 = split_l1(LN), L2 = LN - L1;
+    const bool short_n1 = asym_short_n1(N, M);
+    std::vector<PassParams> v = plan_encode(b, N, short_n1);            // A, BC, D
+    const uint32_t LN = ilog2(N), L1 = split_l1(LN, short_n1), L2 = LN - L1;
     const uint32_t N2 = 1u << L2, dec = (uint32_t)(N / M), N2s = N2 / dec;
     const long long q = (long long)(kM / (2 * N));
     v[1].dst = b.y;
@@ -198,14 +211,14 @@ inline bool shard_supported(size_t N, uint32_t G)
     if (!is_pow2(N) || !is_pow2(G) || G < 2) return false;
     const uint32_t LN = ilog2(N);
     if (LN <= (uint32_t)kMaxLogR || LN > 19) return false;
-    const uint32_t L2 = LN - split_l1(LN);
+    const uint32_t L2 = LN - split_l1(LN, true);
     return (1u << L2) >= G * 1u && ((1u << L2) % G) == 0;
 }
 inline PassParams plan_encode_shard(const Buffers& b, size_t N, uint32_t G, uint32_t rank, int which)
 {
     const uint32_t LN = ilog2(N);
     const long long q = (long long)(kM / (2 * N));
-    const uint32_t L1 = split_l1(LN), L2 = LN - L1;
+    const uint32_t L1 = split_l1(LN, true), L2 = LN - L1;
     const uint32_t N1 = 1u << L1, N2 = 1u << L2;
     PassParams p;
     if (which == 0) {
@@ -242,7 +255,7 @@ inline PassParams plan_encode_shard(const Buffers& b, size_t N, uint32_t G, uint
 inline bool shard_p2p_supported(size_t N, uint32_t G)
 {
     if (!shard_supported(N, G) || G > kMaxPeers) return false;
-    const uint32_t LN = ilog2(N), L1 = split_l1(LN), L2 = LN - L1, lg = ilog2(G);
+    const uint32_t LN = ilog2(N), L1 = split_l1(LN, true), L2 = LN - L1, lg = ilog2(G);
     return L1 >= 5 + lg && L2 >= 5 + lg;
 }
 inline PassParams plan_encode_shard_p2p(const uint32_t* src, uint32_t* const* peers, const uint4* tw, uint32_t pitch_words, uint32_t size_words,
@@ -251,7 +264,7 @@ inline PassParams plan_encode_shard_p2p(const uint32_t* src, uint32_t* const* pe
     Buffers b{const_cast<uint32_t*>(src), nullptr, tw, pitch_words, size_words};
     PassParams p = plan_encode_shard(b, N, G, rank, which);
     if (which == 2) return p;                                       // local, in place
-    const uint32_t LN = ilog2(N), L1 = split_l1(LN), N2 = 1u << (LN - L1);
+    const uint32_t LN = ilog2(N), L1 = split_l1(LN, true), N2 = 1u << (LN - L1);
     p.log_g = ilog2(G);
     for (uint32_t r = 0; r < kMaxPeers; ++r) p.peers[r] = peers[r < G ? r : 0];
     p.dst = peers[rank];
@@ -270,14 +283,14 @@ inline bool ntt_shard_p2p_supported(size_t N, uint32_t G)
     if (!is_pow2(N) || !is_pow2(G) || G < 2 || G > kMaxPeers) return false;
     const uint32_t LN = ilog2(N);
     if (LN <= (uint32_t)kMaxLogR || LN > 20) return false;
-    const uint32_t L1 = split_l1(LN), L2 = LN - L1, lg = ilog2(G);
+    const uint32_t L1 = split_l1(LN, true), L2 = LN - L1, lg = ilog2(G);
     return L1 >= 5 + lg && L2 >= lg;
 }
 inline PassParams plan_ntt_shard_p2p(const uint32_t* src, uint32_t* const* peers, const uint4* tw, uint32_t pitch_words, uint32_t size_words,
                                      size_t N, uint32_t G, uint32_t rank, bool inverse, int which)
 {
     Buffers b{const_cast<uint32_t*>(src), nullptr, tw, pitch_words, size_words};
-    const uint32_t LN = ilog2(N), L1 = split_l1(LN), L2 = LN - L1;
+    const uint32_t LN = ilog2(N), L1 = split_l1(LN, true), L2 = LN - L1;
     const uint32_t N1 = 1u << L1, N2 = 1u << L2;
     const long long p = (long long)(kM / N) * (inverse ? -1 : 1);       // w = g^p
     PassParams a;

@@ -202,7 +202,7 @@ int fastecc_b200_ntt_shard_p2p(uint32_t* const* d_x_peers, uint32_t* const* d_y_
 int fastecc_b200_ntt_shard_pass_p2p(const uint32_t* d_src, uint32_t* const* d_peers, size_t N, int n_ranks, int rank,
                                     size_t SIZE_words, size_t pitch_words, int inverse, int which, void* stream);
 
-/* The decomposition N = N1 * N2 the passes use (csrc/plan.h split_l1, FASTECC_B200_SPLIT honoured), for callers that do the
+/* The decomposition N = N1 * N2 the sharded passes use (csrc/plan.h split_l1, FASTECC_B200_SPLIT honoured), for callers that do the
  * exchange themselves; *fused_exchange_ok: bit 0 = the encode _p2p passes, bit 1 = the NTT _p2p passes support (N, n_ranks).  Fails if N cannot be sharded. */
 int fastecc_b200_shard_geometry(size_t N, int n_ranks, size_t* N1, size_t* N2, int* fused_exchange_ok);
 /* cudaMemcpy2DAsync between pinned host memory and a device buffer (column chunks of a block array), for pipelined
