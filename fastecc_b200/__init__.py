@@ -67,6 +67,9 @@ def lib() -> ctypes.CDLL:
         L.fastecc_b200_rs_decode_recover.argtypes = [vp, vp, sz, sz, vp, sz, vp]; L.fastecc_b200_rs_decode_recover.restype = ci
         L.fastecc_b200_rs_decode_count.argtypes = [vp]; L.fastecc_b200_rs_decode_count.restype = sz
         L.fastecc_b200_rs_decode_free.argtypes = [vp]; L.fastecc_b200_rs_decode_free.restype = None
+        L.fastecc_b200_rs_repair_pattern.argtypes = [sz, sz, vp, sz, vp, sz, vp, ctypes.POINTER(vp)]; L.fastecc_b200_rs_repair_pattern.restype = ci
+        L.fastecc_b200_rs_repair.argtypes = [vp, vp, sz, vp, sz, sz, vp]; L.fastecc_b200_rs_repair.restype = ci
+        L.fastecc_b200_rs_repair_free.argtypes = [vp]; L.fastecc_b200_rs_repair_free.restype = None
         L.fastecc_b200_rs_encode_shard_pass.argtypes = [vp, sz, ci, ci, sz, sz, ci, vp]; L.fastecc_b200_rs_encode_shard_pass.restype = ci
         L.fastecc_b200_rs_encode_shard_pass_p2p.argtypes = [vp, vp, sz, ci, ci, sz, sz, ci, vp]; L.fastecc_b200_rs_encode_shard_pass_p2p.restype = ci
         L.fastecc_b200_ntt_shard_pass_p2p.argtypes = [vp, vp, sz, ci, ci, sz, sz, ci, ci, vp]; L.fastecc_b200_ntt_shard_pass_p2p.restype = ci
@@ -256,6 +259,19 @@ def rs_encode_asym_mixed_dev(t, M: int) -> None:
     N = t.shape[0]); the other rows are undefined afterwards."""
     ptr, N, size, pitch, stream = _dev_args(t)
     _check(lib().fastecc_b200_rs_encode_asym_mixed_dev(ptr, N, M, size, pitch, stream))
+
+
+def rs_repair_dev(data, parity, lost_data, lost_parity) -> None:
+    """Repair a stored stripe in place: data = the N data rows, parity = the M parity rows of rs_encode_asym_mixed_dev (int32
+    CUDA tensors, 16-byte aligned rows with pitches that are multiples of 4 words); lost_data / lost_parity = the lost block
+    numbers (at most M in all).  The lost rows receive their canonical blocks, nothing else is written.  One-shot form of
+    decoder.Repair (which builds the pattern once for any number of stripes)."""
+    from .decoder import Repair
+    r = Repair(data.shape[0], parity.shape[0], lost_data, lost_parity)
+    try:
+        r.repair(data, parity)
+    finally:
+        r.close()
 
 
 def bytes_to_gfp_dev(raw, words=None):

@@ -6,6 +6,7 @@
 #include "byte_recode.h"
 #include "elementwise.h"
 #include "mixed_radix.h"
+#include "repair.h"
 #include <cuda_runtime.h>
 #include <cstdio>
 #include <cstdarg>
@@ -71,7 +72,7 @@ struct SharedBuf {
 // and the destructor records `done` on the caller's stream on every exit path, error returns included.  A user on another
 // stream waits for `done` in acquire(), so two transforms that need the same buffer run one after the other on the device
 // and the buffer is never reallocated under launches that still use it.
-// Lock order: g_host_mu -> packed -> (scratch | mixed, never both at once) -> g_mu.
+// Lock order: g_host_mu -> packed -> repair -> (scratch | mixed, never both at once) -> g_mu.
 class Lease {
 public:
     Lease(SharedBuf* s, cudaStream_t st) : s_(s), st_(st) { if (s_) lk_ = std::unique_lock<std::mutex>(s_->mu); }
@@ -98,6 +99,7 @@ struct Context {
     SharedBuf scratch;   // Y buffer of the two-pass NTT and of the asymmetric encode
     SharedBuf packed;    // repacked copy for unaligned device layouts
     SharedBuf mixed;     // destination of the order-3 / order-9 step of the N = 3 * 2^k, 9 * 2^k transforms
+    SharedBuf repair;    // workspace of fastecc_b200_rs_repair: N + M rows of one column chunk
     DevBuf staging;      // device copy for the host (T**) entry points (serialised by g_host_mu)
     std::map<TableKey, std::vector<TableSlot>> tables;   // one slot per pass of the plan
     bool pin_caller = false;                          // fastecc_b200_pin_host_buffers()
@@ -447,6 +449,38 @@ int shard_pass(Kind kind, const uint32_t* src, uint32_t* const* peers, size_t N,
     return launch_plan(c, plan, st);
 }
 
+// Words per column chunk of a repair: the padded SIZE if the (N + M)-row workspace of it fits in kMaxRepairBytes, else the
+// widest multiple of 4 that does.
+constexpr size_t kMaxRepairBytes = (size_t)4 << 30;
+size_t repair_chunk_words(size_t N, size_t M, size_t size)
+{
+    const size_t w = padded_pitch(size), cap = kMaxRepairBytes / 4 / (N + M) / 4 * 4;
+    return w <= cap ? w : cap;
+}
+
+// The repair of one stripe (DESIGN 3g), once per column chunk [c0, c0 + cols) of the caller's rows: load the data with the lost
+// rows zeroed, encode it, syndromes, inverse order-M transform, split, the forward order-N / order-M transforms of what was lost,
+// scatter into the lost rows.  Transforms of order 1 are the identity and are skipped.
+int repair(Context* c, const fastecc_b200_repair* R, uint32_t* data, size_t dpitch, uint32_t* parity, size_t ppitch, size_t size, cudaStream_t st)
+{
+    const size_t N = R->N, M = R->M, w = repair_chunk_words(N, M, size);
+    Lease ws(&c->repair, st);
+    CUDA_TRY(ws.acquire((N + M) * w * sizeof(uint32_t)));
+    uint32_t* x = ws.ptr();
+    for (size_t c0 = 0; c0 < size; c0 += w) {
+        const size_t cols = size - c0 < w ? size - c0 : w;
+        CUDA_TRY(launch_repair_load(R, data, dpitch, c0, x, w, cols, c->num_sms, st)); g_launches++;
+        if (int rc = encode(c, x, N, M, cols, w, st)) return rc;
+        CUDA_TRY(launch_repair_syndrome(R, parity, ppitch, c0, size, x, w, cols, c->num_sms, st)); g_launches++;
+        if (M > 1) { if (int rc = ntt(c, x, M, cols, w, true, st)) return rc; }
+        CUDA_TRY(launch_repair_split(R, x, w, cols, c->num_sms, st)); g_launches++;
+        if (R->ned && N > 1) { if (int rc = ntt(c, x, N, cols, w, false, st)) return rc; }
+        if (R->nep && M > 1) { if (int rc = ntt(c, x + N * w, M, cols, w, false, st)) return rc; }
+        CUDA_TRY(launch_repair_scatter(R, data, dpitch, parity, ppitch, c0, size, x, w, cols, c->num_sms, st)); g_launches++;
+    }
+    return 0;
+}
+
 } // namespace
 
 // internal accessors for the other translation units of the library (decode.cu)
@@ -488,7 +522,7 @@ void fastecc_b200_shutdown(void)
     if (!g_ctx) return;
     cudaSetDevice(g_ctx->device);
     cudaDeviceSynchronize();
-    g_ctx->scratch.destroy(); g_ctx->packed.destroy(); g_ctx->mixed.destroy(); g_ctx->staging.release();
+    g_ctx->scratch.destroy(); g_ctx->packed.destroy(); g_ctx->mixed.destroy(); g_ctx->repair.destroy(); g_ctx->staging.release();
     for (auto& r : g_ctx->registered) cudaHostUnregister(r.first);
     for (auto& kv : g_ctx->tables) for (auto& sl : kv.second) { sl.buf.release(); if (sl.ready) cudaEventDestroy(sl.ready); }
     if (g_ctx->d_tw) cudaFree(g_ctx->d_tw);
@@ -694,6 +728,21 @@ int fastecc_b200_rs_encode_asym_mixed_dev(uint32_t* d, size_t N, size_t M, size_
 
 int fastecc_b200_rs_encode_asym_mixed(uint32_t** data, size_t N, size_t M, size_t size)
 { return encode_host(data, N, M, size, true, "fastecc_b200_rs_encode_asym_mixed"); }
+
+int fastecc_b200_rs_repair(const fastecc_b200_repair* R, uint32_t* d_data, size_t data_pitch, uint32_t* d_parity, size_t parity_pitch, size_t size, void* stream)
+{
+    const char* who = "fastecc_b200_rs_repair";
+    Context* c = ctx(who);
+    if (!c) return FASTECC_B200_ENOINIT;
+    if (!R) return fail(FASTECC_B200_EINVAL, "%s: null pattern", who);
+    if (int rc = check_rows(d_data, R->N, size, data_pitch, true, who)) return rc;
+    if (int rc = check_rows(d_parity, R->M, size, parity_pitch, true, who)) return rc;
+    const uintptr_t d0 = (uintptr_t)d_data, d1 = d0 + ((R->N - 1) * data_pitch + size) * 4;
+    const uintptr_t p0 = (uintptr_t)d_parity, p1 = p0 + ((R->M - 1) * parity_pitch + size) * 4;
+    if (d0 < p1 && p0 < d1) return fail(FASTECC_B200_EINVAL, "%s: the data and parity buffers overlap", who);
+    if (R->ned + R->nep == 0) return 0;
+    return repair(c, R, d_data, data_pitch, d_parity, parity_pitch, size, (cudaStream_t)stream);
+}
 
 int fastecc_b200_pin_host_buffers(int enable)
 {

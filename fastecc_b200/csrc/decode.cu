@@ -11,9 +11,11 @@
 // polynomials (as word columns), one pairwise product (with the 1/n of the inverse transform folded in) and ONE batched
 // inverse transform.  The Python mirror of the same algorithm is fastecc_b200/decoder.py.  Code words of 3 * 2^k and 9 * 2^k
 // data blocks (fastecc_b200_rs_decode_pattern_mixed, DESIGN 3c / 3e) use the same steps with rho = GF_Root(2N) split by the CRT.
+// The locator part (erasure_locator, declared in locator.h) also serves the repair patterns of repair.cu.
 #include "../../include/fastecc_b200.h"
 #include "gf.cuh"
 #include "mixed_radix.h"
+#include "locator.h"
 #include <cuda_runtime.h>
 #include <vector>
 #include <new>
@@ -51,10 +53,6 @@ __device__ uint32_t invmod(uint32_t x)
 #define FOR_EACH(i, n) for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < (n); i += (size_t)gridDim.x * blockDim.x)
 
 __global__ void iota_kernel(uint32_t* out, size_t n) { FOR_EACH(i, n) out[i] = (uint32_t)i; }
-
-// rho^e, rho = GF_Root(n2), n2 = r * 2^t (r = 1, 3 or 9), split by the CRT: GF_Root(r)^(a2*e mod r) * GF_Root(2^t)^(b2*e mod 2^t),
-// a2 = 2^-t mod r, b2 = r^-1 mod 2^t; GF_Root(2^t)^m = g^(m << log_step) is a power-table entry.  r = 1: a2 = 0, b2 = 1.
-struct LeafRoots { uint32_t r, a2, b2, mask, log_step; uint32_t zeta[9]; };
 
 // Leaves: polynomial g (column g of `polys`, coefficient k in row k, pitch words per row) = prod over its <= 32 points of
 // (x - rho^e); groups beyond the erased set are the constant 1.
@@ -131,11 +129,6 @@ __global__ void gather_scale_kernel(const uint4* __restrict__ code, size_t pitch
     }
 }
 
-struct Scratch {                      // frees what a failed / finished pattern build allocated
-    std::vector<void*> p;
-    ~Scratch() { for (void* q : p) cudaFree(q); }
-    uint32_t* words(size_t n) { void* q = nullptr; if (cudaMalloc(&q, (n ? n : 1) * sizeof(uint32_t)) != cudaSuccess) { cudaGetLastError(); return nullptr; } p.push_back(q); return (uint32_t*)q; }
-};
 inline size_t pad4(size_t n) { return (n + 3) / 4 * 4; }
 
 #define TRY_CUDA(expr) do { cudaError_t e_ = (expr); if (e_ != cudaSuccess) return fail(FASTECC_B200_ECUDA, "%s: %s", #expr, cudaGetErrorString(e_)); } while (0)
@@ -151,10 +144,10 @@ size_t order_above(size_t t)
     return best;
 }
 
-int build_pattern(fastecc_b200_erasures* E, const uint32_t* erased, cudaStream_t st)
+} // namespace
+
+LeafRoots fecc::leaf_roots(size_t n2)
 {
-    const size_t n2 = E->n2, me = E->me;
-    const uint4* tw = context_power_table();
     LeafRoots lr{};
     const Order o = split_order(n2);                                            // n2 = r * 2^t, 2^t <= 2^20
     const CrtSplit ab = crt_split(o.r, o.log2_m);
@@ -164,20 +157,19 @@ int build_pattern(fastecc_b200_erasures* E, const uint32_t* erased, cudaStream_t
         const uint32_t zr = gf::root(lr.r);
         for (uint32_t j = 0; j < 9; ++j) lr.zeta[j] = gf::powmod(zr, j);
     }
-    TRY_CUDA(cudaMalloc((void**)&E->d_pos, n2 * 4));
-    iota_kernel<<<GRID(n2), 256, 0, st>>>(E->d_pos, n2);
-    if (me == 0) return 0;
-    TRY_CUDA(cudaMalloc((void**)&E->d_idx, me * 4));
-    TRY_CUDA(cudaMalloc((void**)&E->d_lv, n2 * 4));
-    TRY_CUDA(cudaMalloc((void**)&E->d_ce, me * 4));
-    TRY_CUDA(cudaMemcpyAsync(E->d_idx, erased, me * 4, cudaMemcpyHostToDevice, st));
-    Scratch tmp;
+    return lr;
+}
+
+int fecc::erasure_locator(size_t n2, const uint32_t* d_idx, size_t me, Scratch& tmp, uint32_t** lv4_out, uint32_t** dl4_out, cudaStream_t st, const char* who)
+{
+    const uint4* tw = context_power_table();
+    const LeafRoots lr = leaf_roots(n2);
     // leaves
     size_t groups = 1; while (groups * kLeaf < me) groups *= 2;
     size_t d = kLeaf, cnt = groups, pitch = pad4(cnt), held = kLeaf + 1;       // held: rows of `polys`
     uint32_t* polys = tmp.words((d + 1) * pitch);
-    if (!polys) return fail(FASTECC_B200_ENOMEM, "fastecc_b200_rs_decode_pattern: out of device memory");
-    leaves_kernel<<<GRID(groups), 256, 0, st>>>(E->d_idx, me, lr, tw, polys, groups, pitch);
+    if (!polys) return fail(FASTECC_B200_ENOMEM, "%s: out of device memory", who);
+    leaves_kernel<<<GRID(groups), 256, 0, st>>>(d_idx, me, lr, tw, polys, groups, pitch);
     // product tree: cnt polynomials of degree <= d  ->  cnt/2 of degree <= 2d.  Batched transforms of order 4d; beyond 2^20
     // (more than 2^19 erasures: code words of 3 * 2^k, 9 * 2^k blocks) the smallest order above the largest actual product
     // degree min(2d, |E|), with the min(d, |E|) + 1 rows that can be nonzero copied in.
@@ -187,7 +179,7 @@ int build_pattern(fastecc_b200_erasures* E, const uint32_t* erased, cudaStream_t
         const size_t half = cnt / 2, hp = pad4(half);
         uint32_t* a = tmp.words(rows * pitch);
         uint32_t* b = tmp.words(rows * hp);
-        if (!a || !b) return fail(FASTECC_B200_ENOMEM, "fastecc_b200_rs_decode_pattern: out of device memory");
+        if (!a || !b) return fail(FASTECC_B200_ENOMEM, "%s: out of device memory", who);
         pad_rows_kernel<<<GRID(rows * pitch), 256, 0, st>>>(polys, pitch, copy, a, pitch, rows, cnt);
         TRY_RC(fastecc_b200_ntt_u32_dev(a, rows, cnt, pitch, 0, st));
         if (hp != half) TRY_CUDA(cudaMemsetAsync(b, 0, rows * hp * sizeof(uint32_t), st));      // pad columns: transformed along, never used
@@ -198,12 +190,31 @@ int build_pattern(fastecc_b200_erasures* E, const uint32_t* erased, cudaStream_t
     // l(rho^m) and D = NTT(t * l_t): two single-column transforms of order n2 (16-byte rows)
     uint32_t* lv4 = tmp.words(n2 * 4);
     uint32_t* dl4 = tmp.words(n2 * 4);
-    if (!lv4 || !dl4) return fail(FASTECC_B200_ENOMEM, "fastecc_b200_rs_decode_pattern: out of device memory");
+    if (!lv4 || !dl4) return fail(FASTECC_B200_ENOMEM, "%s: out of device memory", who);
     size_t ncoef = d + 1 < n2 ? d + 1 : n2;
     if (ncoef > held) ncoef = held;
     locator_columns_kernel<<<GRID(n2), 256, 0, st>>>(polys, pitch, ncoef, lv4, dl4, n2);
     TRY_RC(fastecc_b200_ntt_u32_dev(lv4, n2, 1, 4, 0, st));
     TRY_RC(fastecc_b200_ntt_u32_dev(dl4, n2, 1, 4, 0, st));
+    *lv4_out = lv4; *dl4_out = dl4;
+    return 0;
+}
+
+namespace {
+
+int build_pattern(fastecc_b200_erasures* E, const uint32_t* erased, cudaStream_t st)
+{
+    const size_t n2 = E->n2, me = E->me;
+    TRY_CUDA(cudaMalloc((void**)&E->d_pos, n2 * 4));
+    iota_kernel<<<GRID(n2), 256, 0, st>>>(E->d_pos, n2);
+    if (me == 0) return 0;
+    TRY_CUDA(cudaMalloc((void**)&E->d_idx, me * 4));
+    TRY_CUDA(cudaMalloc((void**)&E->d_lv, n2 * 4));
+    TRY_CUDA(cudaMalloc((void**)&E->d_ce, me * 4));
+    TRY_CUDA(cudaMemcpyAsync(E->d_idx, erased, me * 4, cudaMemcpyHostToDevice, st));
+    Scratch tmp;
+    uint32_t *lv4 = nullptr, *dl4 = nullptr;
+    TRY_RC(erasure_locator(n2, E->d_idx, me, tmp, &lv4, &dl4, st, "fastecc_b200_rs_decode_pattern"));
     finish_pattern_kernel<<<GRID(n2), 256, 0, st>>>(lv4, dl4, E->d_idx, n2, me, E->d_lv, E->d_ce);
     TRY_CUDA(cudaGetLastError());
     TRY_CUDA(cudaStreamSynchronize(st));                                        // the scratch buffers are freed on return

@@ -227,6 +227,59 @@ class CErasurePattern:
             pass
 
 
+class Repair:
+    """Repair of a stored stripe in place through the C ABI (fastecc_b200_rs_repair_pattern / _repair: csrc/repair.cu, DESIGN 3g):
+    the N data rows and M parity rows of EncodeReedSolomon_asym_mixed / rs_encode_asym_mixed_dev (M divides N, M = N included),
+    with the blocks `lost_data` (< N) and `lost_parity` (< M) lost, at most M in all.  The pattern is built on the device once;
+    repair() serves any number of stripes of any SIZE and is asynchronous on the current stream."""
+
+    def __init__(self, N: int, M: int, lost_data=(), lost_parity=()):
+        import ctypes
+        import numpy as np
+        import torch
+        import fastecc_b200 as fe
+        self._fe, self._lib, self._h = fe, fe.lib(), None
+        fe.init(torch.cuda.current_device())
+        lists = []
+        for name, lost in (("lost_data", lost_data), ("lost_parity", lost_parity)):
+            a = np.ascontiguousarray(np.asarray(lost, dtype=np.int64).reshape(-1))
+            if a.size and (a.min() < 0 or a.max() >= (1 << 32)):
+                raise ValueError("%s: block numbers in [0, 2^32)" % name)
+            lists.append(a.astype(np.uint32))
+        d, p = lists
+        h = ctypes.c_void_p()
+        fe._check(self._lib.fastecc_b200_rs_repair_pattern(int(N), int(M), d.ctypes.data, d.size, p.ctypes.data, p.size,
+                                                           torch.cuda.current_stream().cuda_stream, ctypes.byref(h)))
+        self._h, self.N, self.M = h, int(N), int(M)
+        self.lost_data, self.lost_parity = d.tolist(), p.tolist()
+
+    def repair(self, data, parity):
+        """data: [N, S] and parity: [M, S] int32 CUDA tensors (unit word stride), repaired in place."""
+        import torch
+        if self._h is None:
+            raise ValueError("the pattern was closed")
+        for t, rows, name in ((data, self.N, "data"), (parity, self.M, "parity")):
+            if not (t.is_cuda and t.dim() == 2 and t.dtype in (torch.int32, torch.uint32) and t.stride(1) == 1):
+                raise ValueError("%s: expected a 2-D CUDA int32/uint32 tensor with unit stride along the word dimension" % name)
+            if t.shape[0] != rows:
+                raise ValueError("%s has %d rows, the pattern was built for %d" % (name, t.shape[0], rows))
+        if data.shape[1] != parity.shape[1]:
+            raise ValueError("data and parity rows differ in length: %d and %d words" % (data.shape[1], parity.shape[1]))
+        self._fe._check(self._lib.fastecc_b200_rs_repair(self._h, data.data_ptr(), data.stride(0), parity.data_ptr(), parity.stride(0),
+                                                         data.shape[1], torch.cuda.current_stream(data.device).cuda_stream))
+
+    def close(self):
+        if self._h:
+            self._lib.fastecc_b200_rs_repair_free(self._h)
+        self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:            # noqa: BLE001 -- interpreter shutdown
+            pass
+
+
 def decode(code, erased, be=None):
     """One-shot form: build the pattern, recover the erased rows of `code` (destroyed)."""
     return ErasurePattern(code.shape[0], erased, code.device, be).recover(code)

@@ -158,6 +158,28 @@ int    fastecc_b200_rs_decode_recover(const fastecc_b200_erasures* pattern, uint
 size_t fastecc_b200_rs_decode_count(const fastecc_b200_erasures* pattern);        /* n_erased */
 void   fastecc_b200_rs_decode_free(fastecc_b200_erasures* pattern);
 
+/* ---- repair of a stored stripe, in place ---------------------------------------------------------------------------------
+ * The stripe as fastecc_b200_rs_encode_asym_mixed[_dev] leaves it: N data rows and the M parity rows (any (N, M) that encode
+ * accepts, M = N included).  Any n_lost_data + n_lost_parity <= M lost blocks, data and parity alike, are recomputed in place;
+ * the cost follows the stripe (one encode, order-M and order-N transforms), not a 2N-row code word (DESIGN 3g).
+ *   _pattern: everything that depends only on which blocks are lost, built on the device (synchronises the stream).  lost_data /
+ *             lost_parity: HOST arrays, ascending, distinct, below N and M.  Validated in full before anything is allocated.
+ *   _repair:  d_data = N rows (data_pitch_words apart), d_parity = M rows (parity_pitch_words apart), both 16-byte aligned with
+ *             pitches that are multiples of 4 words, not overlapping.  The content of the lost rows is arbitrary, surviving words
+ *             are taken mod P.  On return words [0, SIZE) of every lost row hold the canonical block; nothing else in either buffer
+ *             is written (no surviving row, no pad word beyond SIZE).  Asynchronous on the stream; with nothing lost it returns
+ *             0 without launching anything.  A pattern serves any number of stripes of any SIZE.
+ * Device memory: a workspace of N + M rows of one column chunk, kept by the context like the transforms' scratch buffers, plus
+ * the encode's and the transforms' buffers (N rows of the chunk each).  The chunk is the whole padded SIZE when
+ * (N + M) * ceil4(SIZE) * 4 bytes <= 4 GiB, else the widest multiple of 4 words within that bound, and the repair runs once per
+ * chunk (a 2^19 x 4 KiB stripe is one chunk for every M). */
+typedef struct fastecc_b200_repair fastecc_b200_repair;
+int  fastecc_b200_rs_repair_pattern(size_t N, size_t M, const uint32_t* lost_data, size_t n_lost_data,
+                                    const uint32_t* lost_parity, size_t n_lost_parity, void* stream, fastecc_b200_repair** pattern);
+int  fastecc_b200_rs_repair(const fastecc_b200_repair* pattern, uint32_t* d_data, size_t data_pitch_words,
+                            uint32_t* d_parity, size_t parity_pitch_words, size_t SIZE_words, void* stream);
+void fastecc_b200_rs_repair_free(fastecc_b200_repair* pattern);
+
 /* ---- one transform sharded over several GPUs (one process per GPU; BASELINE config 4) ---------------------------
  * Global block i = l*n_ranks + rank is local block l (data in, parity out).  An encode is: pass 0 on every rank,
  * all-to-all of whole blocks, pass 1, all-to-all, pass 2 -- the exchange is the caller's (fastecc_b200/sharded.py does it

@@ -35,6 +35,19 @@ for N, M, S in ((3 << 12, (3 << 12) // 8, 16), (3 << 11, 1, 1024)):     # the en
     full = torch.from_numpy(a.view(np.int32)).cuda()
     fe.rs_encode_mixed_dev(full)
     assert torch.equal(t[:M], full[::N // M]), ("asym mixed", N, M, S)
+for N, M, S in ((3 << 10, 3 << 6, 1022), (1 << 12, 1 << 12, 16)):         # repair in place (repair.cu's four kernels, a partial last chunk in the first)
+    a = ol.fill_B(o, N, S)
+    data = torch.zeros((N, (S + 3) // 4 * 4), dtype=torch.int32, device="cuda")
+    data[:, :S] = torch.from_numpy(a.view(np.int32)).cuda()
+    par = data.clone()
+    fe.rs_encode_asym_mixed_dev(par[:, :S], M)
+    par = par[:M].clone()
+    want_d, want_p = data.clone(), par.clone()
+    lost_d, lost_p = list(range(0, N, N // (M // 2))), list(range(1, M, 2))
+    data[lost_d, :S] = -1
+    par[lost_p, :S] = -1
+    fe.rs_repair_dev(data[:, :S], par[:, :S], lost_d, lost_p)
+    assert torch.equal(data, want_d) and torch.equal(par, want_p), ("repair", N, M, S)
 raw = torch.randint(0, 256, (64, 4096), dtype=torch.uint8, device="cuda")
 w = fe.bytes_to_gfp_dev(raw)
 assert bool((fe.gfp_to_bytes_dev(w, 1024) == raw).all())

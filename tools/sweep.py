@@ -3,7 +3,8 @@
 encode at N = 2^7 .. 2^19 and forward NTT at N = 2^10 .. 2^20, 4096-byte blocks, CUDA events around `reps` back-to-back
 calls.  Arrays below ~100 MB stay in the 126 MB L2 between calls (marked); the small orders are launch-latency bound.
 Then recoding, decoding, the asymmetric encode, the encode of 3 * 2^k / 9 * 2^k blocks (`encode_mixed`, DESIGN 3e) and
-their encode into fewer parity blocks (`encode_asym_mixed`, DESIGN 3f; `--asym-mixed`: only these).
+their encode into fewer parity blocks (`encode_asym_mixed`, DESIGN 3f; `--asym-mixed`: only these).  `--repair`: only the repair
+of a stored stripe against the 2N-row decoder (DESIGN 3g).
 Prints one JSON line per point."""
 import json
 import os
@@ -185,5 +186,73 @@ def asym_mixed_encode(S):
         torch.cuda.empty_cache()
 
 
+def repair_sweep(S):
+    """Repair of a stored stripe in place (fastecc_b200_rs_repair, DESIGN 3g) with M and M/8 blocks lost, half of them data, half
+    parity, against the same losses through the 2N-row decoder: assemble the code word (data in the even rows, parity in every
+    2(N/M)-th odd row), asym_erasures + CErasurePattern(mixed=True), recover.  Pattern builds are wall-clock times; the repair
+    and the recover are CUDA-event times, two runs each, alternated (the lower figures).  Each line names the card and its
+    power limit, read in the same run."""
+    import time
+    from bench import gpu_identity
+    from fastecc_b200 import decoder
+    card = gpu_identity(torch.cuda.current_device())
+    rng = np.random.default_rng(1)
+    points = [(1 << 19, m) for m in (1 << 19, 1 << 18, 1 << 15, 1 << 13)] + [(3 << 19, 1 << 19), (9 << 18, 1 << 18)]
+    for N, M in points:
+        data = (torch.arange(N * S, device="cuda", dtype=torch.int64) % P).to(torch.int32).view(N, S)
+        torch.cuda.empty_cache()                              # so that no block below lands in (and pins) a cached int64 temporary
+        buf = data.clone()
+        fe.rs_encode_asym_mixed_dev(buf, M)
+        parity = torch.empty((M, S), dtype=torch.int32, device="cuda")
+        parity.copy_(buf[:M])
+        del buf
+        torch.cuda.empty_cache()
+        for lost in (M, M // 8):
+            lost_d = sorted(rng.choice(N, size=lost // 2, replace=False).tolist())
+            lost_p = sorted(rng.choice(M, size=lost - lost // 2, replace=False).tolist())
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            rep = decoder.Repair(N, M, lost_d, lost_p)
+            t_pat = (time.perf_counter() - t0) * 1e3
+            torch.cuda.empty_cache()                          # the 2N-row code word of 9 * 2^18 blocks takes 18 GiB in one piece
+            line = {"op": "repair", "N": N, "M": M, "lost_data": len(lost_d), "lost_parity": len(lost_p), "block_bytes": 4 * S,
+                    "pattern_ms_wall": round(t_pat, 1), "gpu": card["name"], "power_limit_w": card["power_limit_w"]}
+            code = old = None
+            try:
+                t0 = time.perf_counter()
+                code = torch.zeros((2 * N, S), dtype=torch.int32, device="cuda")
+                code[0::2] = data
+                code[1::2 * (N // M)] = parity
+                torch.cuda.synchronize()
+                line["old_assemble_ms_wall"] = round((time.perf_counter() - t0) * 1e3, 1)
+                t0 = time.perf_counter()
+                old = decoder.CErasurePattern(2 * N, decoder.asym_erasures(N, M, lost_d, lost_p), mixed=True)
+                torch.cuda.synchronize()
+                line["old_pattern_ms_wall"] = round((time.perf_counter() - t0) * 1e3, 1)
+            except (torch.OutOfMemoryError, fe.FastEccError) as e:          # the 2N-row route needs about twice the memory
+                line["old_route"] = "out of device memory: %s" % str(e).splitlines()[0][:120]
+                code = old = None
+                torch.cuda.empty_cache()
+            runs, runs_old = [], []
+            for _ in range(2):
+                runs.append(timed(lambda: rep.repair(data, parity), 5))
+                if old is not None:
+                    runs_old.append(timed(lambda: old.recover(code), 3))  # (timing only: the workspace is not a code word after the first call)
+            rep.close()
+            if old is not None:
+                old.close()
+                line.update(old_recover_ms=round(min(runs_old), 4), old_recover_runs=[round(v, 4) for v in runs_old])
+            line.update(ms=round(min(runs), 4), ms_runs=[round(v, 4) for v in runs])
+            print(json.dumps(line), flush=True)
+            del code, old, rep
+            torch.cuda.empty_cache()
+        del data, parity
+        torch.cuda.empty_cache()
+
+
 if __name__ == "__main__":
+    if "--repair" in sys.argv:                                # only the repair lines
+        fe.init(0)
+        repair_sweep(1024)
+        sys.exit(0)
     sys.exit(main())
