@@ -1,5 +1,5 @@
 // extern "C" boundary of fastecc_b200 (include/fastecc_b200.h): context, planning, launches, host<->device staging.
-#include "../../include/fastecc_b200.h"
+#include "context.h"
 #include "plan.h"
 #include "ntt_pass.h"
 #include "small_dft.h"
@@ -24,7 +24,6 @@ thread_local char g_err[512] = "no error";
 }
 
 namespace fecc {
-// Records the message for fastecc_b200_last_error() (per thread) and returns `code`; shared with decode.cu.
 int fail(int code, const char* fmt, ...)
 {
     va_list ap; va_start(ap, fmt); vsnprintf(g_err, sizeof g_err, fmt, ap); va_end(ap);
@@ -114,9 +113,6 @@ std::mutex g_mu;          // guards g_ctx and the table cache (short critical se
 std::mutex g_host_mu;     // held by the host (T**) entry points for their whole duration: they share the staging buffer, three streams and the chunk events
 std::atomic<unsigned long long> g_launches{0};
 
-#define CUDA_TRY(expr) do { cudaError_t e_ = (expr); if (e_ != cudaSuccess) \
-    return fail(e_ == cudaErrorMemoryAllocation ? FASTECC_B200_ENOMEM : FASTECC_B200_ECUDA, "%s: %s", #expr, cudaGetErrorString(e_)); } while (0)
-
 // The live context, or nullptr after recording the ENOINIT message.
 Context* ctx(const char* who)
 {
@@ -161,16 +157,16 @@ void pin_caller_array(Context* c, void* base, size_t bytes)
 {
     if (!c->pin_caller || bytes < ((size_t)32 << 20)) return;
     cudaPointerAttributes at;
-    if (cudaPointerGetAttributes(&at, base) != cudaSuccess) { cudaGetLastError(); return; }
+    if (cudaPointerGetAttributes(&at, base) != cudaSuccess) { clear_cuda_error(); return; }
     if (at.type != cudaMemoryTypeUnregistered) return;                      // already pinned (by us earlier, or by the caller)
     char* b = (char*)base;
     for (size_t i = 0; i < c->registered.size();) {                         // a stale, overlapping registration (the caller re-allocated): drop it
         auto& r = c->registered[i];
-        if (b < r.first + r.second && r.first < b + bytes) { cudaHostUnregister(r.first); cudaGetLastError(); r = c->registered.back(); c->registered.pop_back(); }
+        if (b < r.first + r.second && r.first < b + bytes) { cudaHostUnregister(r.first); clear_cuda_error(); r = c->registered.back(); c->registered.pop_back(); }
         else ++i;
     }
     if (cudaHostRegister(base, bytes, cudaHostRegisterDefault) == cudaSuccess) c->registered.emplace_back(b, bytes);
-    else cudaGetLastError();
+    else clear_cuda_error();
 }
 
 // Stage tables of `plan` under cache key `key`: built on first use (a block enters the cache only once it is allocated and
@@ -483,7 +479,6 @@ int repair(Context* c, const fastecc_b200_repair* R, uint32_t* data, size_t dpit
 
 } // namespace
 
-// internal accessors for the other translation units of the library (decode.cu)
 namespace fecc {
 const uint4* context_power_table() { return g_ctx ? g_ctx->d_tw : nullptr; }
 int context_num_sms() { return g_ctx ? g_ctx->num_sms : 0; }
@@ -685,7 +680,7 @@ void* fastecc_b200_dev_alloc(size_t bytes)
 {
     if (!ctx("fastecc_b200_dev_alloc")) return nullptr;
     void* p = nullptr;
-    if (cudaMalloc(&p, bytes) != cudaSuccess) { cudaGetLastError(); fail(FASTECC_B200_ENOMEM, "fastecc_b200_dev_alloc: cudaMalloc(%zu) failed", bytes); return nullptr; }
+    if (cudaMalloc(&p, bytes) != cudaSuccess) { clear_cuda_error(); fail(FASTECC_B200_ENOMEM, "fastecc_b200_dev_alloc: cudaMalloc(%zu) failed", bytes); return nullptr; }
     return p;
 }
 void fastecc_b200_dev_free(void* p) { if (p) cudaFree(p); }
@@ -751,7 +746,7 @@ int fastecc_b200_pin_host_buffers(int enable)
     g_ctx->pin_caller = enable != 0;
     if (!enable) {                                                          // turning it off also releases what was page-locked so far
         CUDA_TRY(cudaDeviceSynchronize());
-        for (auto& r : g_ctx->registered) { cudaHostUnregister(r.first); cudaGetLastError(); }
+        for (auto& r : g_ctx->registered) { cudaHostUnregister(r.first); clear_cuda_error(); }
         g_ctx->registered.clear();
     }
     return 0;

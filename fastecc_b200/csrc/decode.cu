@@ -12,19 +12,9 @@
 // inverse transform.  The Python mirror of the same algorithm is fastecc_b200/decoder.py.  Code words of 3 * 2^k and 9 * 2^k
 // data blocks (fastecc_b200_rs_decode_pattern_mixed, DESIGN 3c / 3e) use the same steps with rho = GF_Root(2N) split by the CRT.
 // The locator part (erasure_locator, declared in locator.h) also serves the repair patterns of repair.cu.
-#include "../../include/fastecc_b200.h"
-#include "gf.cuh"
 #include "mixed_radix.h"
 #include "locator.h"
-#include <cuda_runtime.h>
-#include <vector>
 #include <new>
-
-namespace fecc {
-const uint4* context_power_table();          // api.cu: g^e, e in [0, 2^20), or nullptr before fastecc_b200_init()
-int          context_num_sms();
-int          fail(int code, const char* fmt, ...);      // api.cu: records the message for fastecc_b200_last_error()
-}
 
 struct fastecc_b200_erasures {
     size_t n2 = 0, me = 0;
@@ -32,6 +22,7 @@ struct fastecc_b200_erasures {
     uint32_t* d_lv = nullptr;        // [n2]  l(rho^m): zero exactly on the erased rows
     uint32_t* d_ce = nullptr;        // [me]  1 / (2N * D[e])
     uint32_t* d_pos = nullptr;       // [n2]  0, 1, 2, ...: the constants of the formal derivative
+    fecc::DeviceArrays mem;          // owns the arrays above
 };
 
 namespace {
@@ -39,27 +30,16 @@ namespace {
 using namespace fecc;
 constexpr uint32_t P = gf::P;
 constexpr uint32_t kLeaf = 32;       // points per leaf polynomial
+constexpr size_t kMaxGrid = 8192;    // blocks of the pattern kernels
 
-__device__ __forceinline__ uint32_t mulmod(uint32_t a, uint32_t b) { return (uint32_t)(((uint64_t)a * b) % P); }
-__device__ __forceinline__ uint32_t submod(uint32_t a, uint32_t b) { return a >= b ? a - b : a + (P - b); }
-__device__ uint32_t invmod(uint32_t x)
-{
-    uint32_t r = 1;
-    for (uint32_t e = P - 2; e; e >>= 1) { if (e & 1u) r = mulmod(r, x); x = mulmod(x, x); }
-    return r;
-}
-
-#define GRID(n) (unsigned)(((n) + 255) / 256 < 8192 ? ((n) + 255) / 256 : 8192)
-#define FOR_EACH(i, n) for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < (n); i += (size_t)gridDim.x * blockDim.x)
-
-__global__ void iota_kernel(uint32_t* out, size_t n) { FOR_EACH(i, n) out[i] = (uint32_t)i; }
+__global__ void iota_kernel(uint32_t* out, size_t n) { FOR_GRID(size_t, i, n) out[i] = (uint32_t)i; }
 
 // Leaves: polynomial g (column g of `polys`, coefficient k in row k, pitch words per row) = prod over its <= 32 points of
 // (x - rho^e); groups beyond the erased set are the constant 1.
 __global__ void leaves_kernel(const uint32_t* __restrict__ idx, size_t me, LeafRoots L, const uint4* __restrict__ tw,
                               uint32_t* __restrict__ polys, size_t groups, size_t pitch)
 {
-    FOR_EACH(g, groups) {
+    FOR_GRID(size_t, g, groups) {
         uint32_t c[kLeaf + 1];
 #pragma unroll
         for (uint32_t k = 0; k <= kLeaf; ++k) c[k] = k == 0 ? 1u : 0u;
@@ -68,12 +48,11 @@ __global__ void leaves_kernel(const uint32_t* __restrict__ idx, size_t me, LeafR
             const size_t e = g * kLeaf + t;
             if (e >= me) break;
             const uint32_t pos = idx[e];
-            uint32_t r = tw[(size_t)((L.b2 * pos) & L.mask) << L.log_step].x;        // rho^e
-            if (L.r > 1) r = mulmod(r, L.zeta[(L.a2 * (pos % L.r)) % L.r]);
+            const uint32_t r = rho_pow(L, tw, pos);
             ++deg;
 #pragma unroll
-            for (int k = kLeaf; k >= 1; --k) if ((uint32_t)k <= deg) c[k] = submod(c[k - 1], mulmod(c[k], r));       // c(x) * (x - r)
-            c[0] = submod(0u, mulmod(c[0], r));
+            for (int k = kLeaf; k >= 1; --k) if ((uint32_t)k <= deg) c[k] = gf::sub(c[k - 1], gf::mulmod(c[k], r));       // c(x) * (x - r)
+            c[0] = gf::sub(0u, gf::mulmod(c[0], r));
         }
 #pragma unroll
         for (uint32_t k = 0; k <= kLeaf; ++k) polys[k * pitch + g] = c[k];
@@ -83,15 +62,15 @@ __global__ void leaves_kernel(const uint32_t* __restrict__ idx, size_t me, LeafR
 // b[r][c] = a[r][2c] * a[r][2c+1] * scale   (point-wise product of neighbouring polynomials in the transform domain)
 __global__ void pairmul_kernel(const uint32_t* __restrict__ a, size_t a_pitch, uint32_t* __restrict__ b, size_t b_pitch, size_t rows, size_t cols_out, uint32_t scale)
 {
-    FOR_EACH(i, rows * cols_out) {
+    FOR_GRID(size_t, i, rows * cols_out) {
         const size_t r = i / cols_out, c = i - r * cols_out;
-        b[r * b_pitch + c] = mulmod(mulmod(a[r * a_pitch + 2 * c], a[r * a_pitch + 2 * c + 1]), scale);
+        b[r * b_pitch + c] = gf::mulmod(gf::mulmod(a[r * a_pitch + 2 * c], a[r * a_pitch + 2 * c + 1]), scale);
     }
 }
 // dst (rows_dst x cols, zero padded) <- rows [0, rows_src) of src
 __global__ void pad_rows_kernel(const uint32_t* __restrict__ src, size_t src_pitch, size_t rows_src, uint32_t* __restrict__ dst, size_t dst_pitch, size_t rows_dst, size_t cols)
 {
-    FOR_EACH(i, rows_dst * dst_pitch) {
+    FOR_GRID(size_t, i, rows_dst * dst_pitch) {
         const size_t r = i / dst_pitch, c = i - r * dst_pitch;
         dst[i] = (r < rows_src && c < cols) ? src[r * src_pitch + c] : 0u;
     }
@@ -99,18 +78,18 @@ __global__ void pad_rows_kernel(const uint32_t* __restrict__ src, size_t src_pit
 // column 0 of a pitched array -> two pitched single-column arrays: l_t and t * l_t
 __global__ void locator_columns_kernel(const uint32_t* __restrict__ polys, size_t pitch, size_t ncoef, uint32_t* __restrict__ lv, uint32_t* __restrict__ dl, size_t n2)
 {
-    FOR_EACH(t, n2) {
+    FOR_GRID(size_t, t, n2) {
         const uint32_t c = t < ncoef ? polys[t * pitch] : 0u;
         lv[t * 4] = c; lv[t * 4 + 1] = 0; lv[t * 4 + 2] = 0; lv[t * 4 + 3] = 0;
-        dl[t * 4] = mulmod(c, (uint32_t)(t % P)); dl[t * 4 + 1] = 0; dl[t * 4 + 2] = 0; dl[t * 4 + 3] = 0;
+        dl[t * 4] = gf::mulmod(c, (uint32_t)(t % P)); dl[t * 4 + 1] = 0; dl[t * 4 + 2] = 0; dl[t * 4 + 3] = 0;
     }
 }
 __global__ void finish_pattern_kernel(const uint32_t* __restrict__ lv4, const uint32_t* __restrict__ dl4, const uint32_t* __restrict__ idx, size_t n2, size_t me,
                                       uint32_t* __restrict__ lv, uint32_t* __restrict__ ce)
 {
-    FOR_EACH(i, n2) {
+    FOR_GRID(size_t, i, n2) {
         lv[i] = lv4[i * 4];
-        if (i < me) ce[i] = invmod(mulmod(dl4[(size_t)idx[i] * 4], (uint32_t)(n2 % P)));       // 1 / (2N * D[e])
+        if (i < me) ce[i] = gf::inv(gf::mulmod(dl4[(size_t)idx[i] * 4], (uint32_t)(n2 % P)));       // 1 / (2N * D[e])
     }
 }
 // out row i = code row idx[i] * ce[i]  (16-byte chunks)
@@ -123,16 +102,13 @@ __global__ void gather_scale_kernel(const uint4* __restrict__ code, size_t pitch
         uint4* dst = out + row * out_pitch4;
         for (uint32_t k = threadIdx.x; k < s4; k += blockDim.x) {
             uint4 v = src[k];
-            v.x = mulmod(v.x % P, c); v.y = mulmod(v.y % P, c); v.z = mulmod(v.z % P, c); v.w = mulmod(v.w % P, c);
+            v.x = gf::mulmod(v.x % P, c); v.y = gf::mulmod(v.y % P, c); v.z = gf::mulmod(v.z % P, c); v.w = gf::mulmod(v.w % P, c);
             dst[k] = v;
         }
     }
 }
 
 inline size_t pad4(size_t n) { return (n + 3) / 4 * 4; }
-
-#define TRY_CUDA(expr) do { cudaError_t e_ = (expr); if (e_ != cudaSuccess) return fail(FASTECC_B200_ECUDA, "%s: %s", #expr, cudaGetErrorString(e_)); } while (0)
-#define TRY_RC(expr) do { int rc_ = (expr); if (rc_) return rc_; } while (0)
 
 // The smallest transform order of the library (2^a, 3 * 2^a or 9 * 2^a with 2^a <= 2^20) above t; 0 if there is none.
 size_t order_above(size_t t)
@@ -160,16 +136,16 @@ LeafRoots fecc::leaf_roots(size_t n2)
     return lr;
 }
 
-int fecc::erasure_locator(size_t n2, const uint32_t* d_idx, size_t me, Scratch& tmp, uint32_t** lv4_out, uint32_t** dl4_out, cudaStream_t st, const char* who)
+int fecc::erasure_locator(size_t n2, const uint32_t* d_idx, size_t me, DeviceArrays& tmp, uint32_t** lv4_out, uint32_t** dl4_out, cudaStream_t st, const char* who)
 {
     const uint4* tw = context_power_table();
     const LeafRoots lr = leaf_roots(n2);
     // leaves
     size_t groups = 1; while (groups * kLeaf < me) groups *= 2;
     size_t d = kLeaf, cnt = groups, pitch = pad4(cnt), held = kLeaf + 1;       // held: rows of `polys`
-    uint32_t* polys = tmp.words((d + 1) * pitch);
+    uint32_t* polys = tmp.alloc<uint32_t>((d + 1) * pitch);
     if (!polys) return fail(FASTECC_B200_ENOMEM, "%s: out of device memory", who);
-    leaves_kernel<<<GRID(groups), 256, 0, st>>>(d_idx, me, lr, tw, polys, groups, pitch);
+    leaves_kernel<<<grid_size(groups, kMaxGrid), 256, 0, st>>>(d_idx, me, lr, tw, polys, groups, pitch);
     // product tree: cnt polynomials of degree <= d  ->  cnt/2 of degree <= 2d.  Batched transforms of order 4d; beyond 2^20
     // (more than 2^19 erasures: code words of 3 * 2^k, 9 * 2^k blocks) the smallest order above the largest actual product
     // degree min(2d, |E|), with the min(d, |E|) + 1 rows that can be nonzero copied in.
@@ -177,23 +153,23 @@ int fecc::erasure_locator(size_t n2, const uint32_t* d_idx, size_t me, Scratch& 
         size_t rows = 4 * d, copy = d + 1;
         if (rows > gf::M) { rows = order_above(2 * d < me ? 2 * d : me); copy = (d < me ? d : me) + 1; }
         const size_t half = cnt / 2, hp = pad4(half);
-        uint32_t* a = tmp.words(rows * pitch);
-        uint32_t* b = tmp.words(rows * hp);
+        uint32_t* a = tmp.alloc<uint32_t>(rows * pitch);
+        uint32_t* b = tmp.alloc<uint32_t>(rows * hp);
         if (!a || !b) return fail(FASTECC_B200_ENOMEM, "%s: out of device memory", who);
-        pad_rows_kernel<<<GRID(rows * pitch), 256, 0, st>>>(polys, pitch, copy, a, pitch, rows, cnt);
+        pad_rows_kernel<<<grid_size(rows * pitch, kMaxGrid), 256, 0, st>>>(polys, pitch, copy, a, pitch, rows, cnt);
         TRY_RC(fastecc_b200_ntt_u32_dev(a, rows, cnt, pitch, 0, st));
-        if (hp != half) TRY_CUDA(cudaMemsetAsync(b, 0, rows * hp * sizeof(uint32_t), st));      // pad columns: transformed along, never used
-        pairmul_kernel<<<GRID(rows * half), 256, 0, st>>>(a, pitch, b, hp, rows, half, gf::inv((uint32_t)rows));
+        if (hp != half) CUDA_TRY(cudaMemsetAsync(b, 0, rows * hp * sizeof(uint32_t), st));      // pad columns: transformed along, never used
+        pairmul_kernel<<<grid_size(rows * half, kMaxGrid), 256, 0, st>>>(a, pitch, b, hp, rows, half, gf::inv((uint32_t)rows));
         TRY_RC(fastecc_b200_ntt_u32_dev(b, rows, half, hp, 1, st));
         polys = b; pitch = hp; cnt = half; d *= 2; held = rows;                // rows [0, min(d, |E|)] of b hold the products
     }
     // l(rho^m) and D = NTT(t * l_t): two single-column transforms of order n2 (16-byte rows)
-    uint32_t* lv4 = tmp.words(n2 * 4);
-    uint32_t* dl4 = tmp.words(n2 * 4);
+    uint32_t* lv4 = tmp.alloc<uint32_t>(n2 * 4);
+    uint32_t* dl4 = tmp.alloc<uint32_t>(n2 * 4);
     if (!lv4 || !dl4) return fail(FASTECC_B200_ENOMEM, "%s: out of device memory", who);
     size_t ncoef = d + 1 < n2 ? d + 1 : n2;
     if (ncoef > held) ncoef = held;
-    locator_columns_kernel<<<GRID(n2), 256, 0, st>>>(polys, pitch, ncoef, lv4, dl4, n2);
+    locator_columns_kernel<<<grid_size(n2, kMaxGrid), 256, 0, st>>>(polys, pitch, ncoef, lv4, dl4, n2);
     TRY_RC(fastecc_b200_ntt_u32_dev(lv4, n2, 1, 4, 0, st));
     TRY_RC(fastecc_b200_ntt_u32_dev(dl4, n2, 1, 4, 0, st));
     *lv4_out = lv4; *dl4_out = dl4;
@@ -202,22 +178,21 @@ int fecc::erasure_locator(size_t n2, const uint32_t* d_idx, size_t me, Scratch& 
 
 namespace {
 
-int build_pattern(fastecc_b200_erasures* E, const uint32_t* erased, cudaStream_t st)
+int build_pattern(fastecc_b200_erasures* E, const uint32_t* erased, cudaStream_t st, const char* who)
 {
     const size_t n2 = E->n2, me = E->me;
-    TRY_CUDA(cudaMalloc((void**)&E->d_pos, n2 * 4));
-    iota_kernel<<<GRID(n2), 256, 0, st>>>(E->d_pos, n2);
+    E->d_pos = E->mem.alloc<uint32_t>(n2);
+    if (me) { E->d_idx = E->mem.alloc<uint32_t>(me); E->d_lv = E->mem.alloc<uint32_t>(n2); E->d_ce = E->mem.alloc<uint32_t>(me); }
+    if (E->mem.failed) return fail(FASTECC_B200_ENOMEM, "%s: out of device memory", who);
+    iota_kernel<<<grid_size(n2, kMaxGrid), 256, 0, st>>>(E->d_pos, n2);
     if (me == 0) return 0;
-    TRY_CUDA(cudaMalloc((void**)&E->d_idx, me * 4));
-    TRY_CUDA(cudaMalloc((void**)&E->d_lv, n2 * 4));
-    TRY_CUDA(cudaMalloc((void**)&E->d_ce, me * 4));
-    TRY_CUDA(cudaMemcpyAsync(E->d_idx, erased, me * 4, cudaMemcpyHostToDevice, st));
-    Scratch tmp;
+    CUDA_TRY(cudaMemcpyAsync(E->d_idx, erased, me * 4, cudaMemcpyHostToDevice, st));
+    DeviceArrays tmp;
     uint32_t *lv4 = nullptr, *dl4 = nullptr;
-    TRY_RC(erasure_locator(n2, E->d_idx, me, tmp, &lv4, &dl4, st, "fastecc_b200_rs_decode_pattern"));
-    finish_pattern_kernel<<<GRID(n2), 256, 0, st>>>(lv4, dl4, E->d_idx, n2, me, E->d_lv, E->d_ce);
-    TRY_CUDA(cudaGetLastError());
-    TRY_CUDA(cudaStreamSynchronize(st));                                        // the scratch buffers are freed on return
+    TRY_RC(erasure_locator(n2, E->d_idx, me, tmp, &lv4, &dl4, st, who));
+    finish_pattern_kernel<<<grid_size(n2, kMaxGrid), 256, 0, st>>>(lv4, dl4, E->d_idx, n2, me, E->d_lv, E->d_ce);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaStreamSynchronize(st));                                        // the scratch buffers are freed on return
     return 0;
 }
 
@@ -232,13 +207,12 @@ int make_pattern(size_t n_rows, const uint32_t* erased, size_t n_erased, void* s
                                                : "%s: the code word must have 2N = 2 .. 2^20 rows (a power of two), got %zu", who, n_rows);
     if (n_erased > n_rows / 2) return fail(FASTECC_B200_EINVAL, "%s: at most N = %zu of the 2N rows can be erased, got %zu", who, n_rows / 2, n_erased);
     if (n_erased && !erased) return fail(FASTECC_B200_EINVAL, "%s: null position list", who);
-    for (size_t i = 0; i < n_erased; ++i)
-        if (erased[i] >= n_rows || (i && erased[i] <= erased[i - 1])) return fail(FASTECC_B200_EINVAL, "%s: erased positions must be ascending, distinct and below %zu", who, n_rows);
+    if (!ascending_below(erased, n_erased, n_rows)) return fail(FASTECC_B200_EINVAL, "%s: erased positions must be ascending, distinct and below %zu", who, n_rows);
     fastecc_b200_erasures* E = new (std::nothrow) fastecc_b200_erasures;
     if (!E) return fail(FASTECC_B200_ENOMEM, "%s: out of host memory", who);
     E->n2 = n_rows; E->me = n_erased;
-    const int rc = build_pattern(E, erased, (cudaStream_t)stream);
-    if (rc) { fastecc_b200_rs_decode_free(E); return rc; }
+    const int rc = build_pattern(E, erased, (cudaStream_t)stream, who);
+    if (rc) { delete E; return rc; }
     *out = E;
     return 0;
 }
@@ -269,17 +243,12 @@ int fastecc_b200_rs_decode_recover(const fastecc_b200_erasures* E, uint32_t* d_c
     const unsigned grid = (unsigned)(E->me < (size_t)fecc::context_num_sms() * 8 ? E->me : (size_t)fecc::context_num_sms() * 8);
     gather_scale_kernel<<<grid, 256, 0, st>>>(reinterpret_cast<const uint4*>(d_code), pitch / 4, E->d_idx, E->d_ce, reinterpret_cast<uint4*>(d_out), out_pitch / 4,
                                               E->me, (uint32_t)((size + 3) / 4));
-    TRY_CUDA(cudaGetLastError());
+    CUDA_TRY(cudaGetLastError());
     return 0;
 }
 
 size_t fastecc_b200_rs_decode_count(const fastecc_b200_erasures* E) { return E ? E->me : 0; }
 
-void fastecc_b200_rs_decode_free(fastecc_b200_erasures* E)
-{
-    if (!E) return;
-    cudaFree(E->d_idx); cudaFree(E->d_lv); cudaFree(E->d_ce); cudaFree(E->d_pos);
-    delete E;
-}
+void fastecc_b200_rs_decode_free(fastecc_b200_erasures* E) { delete E; }          // null-safe
 
 } // extern "C"

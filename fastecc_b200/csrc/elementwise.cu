@@ -3,48 +3,36 @@
 // (the shape of the reference's scaling loop, RS.cpp:51-59, with an arbitrary constant per block).  The first two work on
 // short vectors (one value per block); row_scale streams the block array once: HBM-bound, 16-byte accesses.
 #include "elementwise.h"
+#include "context.h"
 #include "gf.cuh"
 
 namespace fecc {
 
-__device__ __forceinline__ uint32_t mulmod_dev(uint32_t a, uint32_t b) { return (uint32_t)(((uint64_t)a * b) % gf::P); }
-
 __global__ void gf_mul_kernel(const uint32_t* __restrict__ a, const uint32_t* __restrict__ b, uint32_t* __restrict__ out, size_t n)
 {
-    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) out[i] = mulmod_dev(a[i], b[i]);
+    FOR_GRID(size_t, i, n) out[i] = gf::mulmod(a[i], b[i]);
 }
 __global__ void gf_inv_kernel(const uint32_t* __restrict__ a, uint32_t* __restrict__ out, size_t n)
 {
-    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-        uint32_t x = a[i] % gf::P, r = 1;
-        for (uint32_t e = gf::P - 2; e; e >>= 1) { if (e & 1u) r = mulmod_dev(r, x); x = mulmod_dev(x, x); }
-        out[i] = a[i] % gf::P ? r : 0u;
+    FOR_GRID(size_t, i, n) {
+        const uint32_t x = a[i] % gf::P;
+        out[i] = x ? gf::inv(x) : 0u;
     }
 }
 
 // One CTA per row (grid-stride over rows): thread 0 turns the row's constant into its Barrett/Shoup triple
-// (two 64-by-32 divisions, gf::make_tw on the host), every thread then multiplies 16-byte chunks with gf::mul.
+// (gf::make_tw: two 64-by-32 divisions), every thread then multiplies 16-byte chunks with gf::mul4.
 __global__ void __launch_bounds__(256) row_scale_kernel(uint4* __restrict__ d, size_t n_rows, uint32_t s4, uint32_t pitch4, const uint32_t* __restrict__ consts)
 {
     __shared__ uint32_t tw[3];
     const uint32_t zero = gf::opaque_zero();
     for (size_t row = blockIdx.x; row < n_rows; row += gridDim.x) {
         __syncthreads();
-        if (threadIdx.x == 0) {
-            const uint32_t w = consts[row] % gf::P;
-            const uint64_t n1 = (uint64_t)w << 32;
-            const uint64_t whi = n1 / gf::P, rem = n1 % gf::P;
-            tw[0] = w; tw[1] = (uint32_t)whi; tw[2] = (uint32_t)((rem << 32) / gf::P);
-        }
+        if (threadIdx.x == 0) { const gf::Tw t = gf::make_tw(consts[row] % gf::P); tw[0] = t.w; tw[1] = t.whi; tw[2] = t.wlo; }
         __syncthreads();
-        const uint32_t w = tw[0], whi = tw[1], wlo = tw[2];
+        const uint4 t = make_uint4(tw[0], tw[1], tw[2], 0u);
         uint4* r = d + row * pitch4;
-        for (uint32_t c = threadIdx.x; c < s4; c += blockDim.x) {
-            uint4 v = r[c];
-            v.x = gf::canon(gf::mul(v.x, w, whi, wlo, zero)); v.y = gf::canon(gf::mul(v.y, w, whi, wlo, zero));
-            v.z = gf::canon(gf::mul(v.z, w, whi, wlo, zero)); v.w = gf::canon(gf::mul(v.w, w, whi, wlo, zero));
-            r[c] = v;
-        }
+        for (uint32_t c = threadIdx.x; c < s4; c += blockDim.x) r[c] = gf::canon4(gf::mul4(r[c], t, zero));
     }
 }
 
@@ -84,13 +72,13 @@ cudaError_t launch_shard_barrier(uint32_t* const* host_peers, uint32_t n_ranks, 
 cudaError_t launch_gf_mul(const uint32_t* a, const uint32_t* b, uint32_t* out, size_t n, cudaStream_t st)
 {
     if (!n) return cudaSuccess;
-    gf_mul_kernel<<<(unsigned)((n + 255) / 256 < 4096 ? (n + 255) / 256 : 4096), 256, 0, st>>>(a, b, out, n);
+    gf_mul_kernel<<<grid_size(n, 4096), 256, 0, st>>>(a, b, out, n);
     return cudaGetLastError();
 }
 cudaError_t launch_gf_inv(const uint32_t* a, uint32_t* out, size_t n, cudaStream_t st)
 {
     if (!n) return cudaSuccess;
-    gf_inv_kernel<<<(unsigned)((n + 255) / 256 < 4096 ? (n + 255) / 256 : 4096), 256, 0, st>>>(a, out, n);
+    gf_inv_kernel<<<grid_size(n, 4096), 256, 0, st>>>(a, out, n);
     return cudaGetLastError();
 }
 cudaError_t launch_row_scale(uint32_t* d, size_t n_rows, uint32_t s4, uint32_t pitch4, const uint32_t* consts, int num_sms, cudaStream_t st)

@@ -148,12 +148,28 @@ GF_HD uint32_t opaque_zero()
 
 GF_HD uint32_t canon(uint32_t x) { return x >= P ? x - P : x; }
 
-// ---- host-only helpers (table generation, plan constants) --------------------------------------------------------
-inline uint32_t mulmod(uint32_t a, uint32_t b) { return (uint32_t)(((uint64_t)a * b) % P); }
-inline uint32_t powmod(uint32_t x, uint64_t n) { uint32_t r = 1; for (; n; n >>= 1) { if (n & 1) r = mulmod(r, x); x = mulmod(x, x); } return r; }
+// a + b and a - b of canonical residues
+GF_HD uint32_t add(uint32_t a, uint32_t b) { const uint32_t s = a + b; return (s < a || s >= P) ? s - P : s; }
+GF_HD uint32_t sub(uint32_t a, uint32_t b) { return a >= b ? a - b : a + (P - b); }
+
+#if defined(__CUDACC__)
+// The product by a triple t = {w, Whi, Wlo} (a power-table entry or a per-row constant as a uint4, whose .w is unused; a kernel
+// constant as a uint32_t[3]), canonical; and the four-lane forms: mul4 leaves each lane in [0, P] like mul(), canon4 reduces.
+GF_HD uint32_t mulc(uint32_t b, uint4 t, uint32_t zero = 0) { return canon(mul(b, t.x, t.y, t.z, zero)); }
+GF_HD uint32_t mulc(uint32_t b, const uint32_t (&t)[3], uint32_t zero = 0) { return canon(mul(b, t[0], t[1], t[2], zero)); }
+GF_HD uint4 mul4(uint4 v, uint4 t, uint32_t zero = 0)
+{
+    return make_uint4(mul(v.x, t.x, t.y, t.z, zero), mul(v.y, t.x, t.y, t.z, zero), mul(v.z, t.x, t.y, t.z, zero), mul(v.w, t.x, t.y, t.z, zero));
+}
+GF_HD uint4 canon4(uint4 v) { return make_uint4(canon(v.x), canon(v.y), canon(v.z), canon(v.w)); }
+#endif
+
+// ---- products by arbitrary operands (tables, plan constants, the pattern builds of the erasure code) ----------------
+GF_HD uint32_t mulmod(uint32_t a, uint32_t b) { return (uint32_t)(((uint64_t)a * b) % P); }
+GF_HD uint32_t powmod(uint32_t x, uint64_t n) { uint32_t r = 1; for (; n; n >>= 1) { if (n & 1) r = mulmod(r, x); x = mulmod(x, x); } return r; }
 inline uint32_t root(uint32_t n) { return powmod(GEN, (P - 1) / n); }        // GF_Root, GF(p).cpp:267-276
-inline uint32_t inv(uint32_t x)  { return powmod(x, P - 2); }                // GF_Inv,  GF(p).cpp:293-297
-inline Tw make_tw(uint32_t w)            // {w, floor(w*2^64/P)} by two 64/32 long-division steps
+GF_HD uint32_t inv(uint32_t x)  { return powmod(x, P - 2); }                 // GF_Inv,  GF(p).cpp:293-297
+GF_HD Tw make_tw(uint32_t w)             // {w, floor(w*2^64/P)} by two 64/32 long-division steps
 {
     const uint64_t n1 = (uint64_t)w << 32;
     const uint64_t whi = n1 / P, rem = n1 % P;

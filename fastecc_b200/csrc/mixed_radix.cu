@@ -12,6 +12,7 @@
 // so it comes from a 9-entry constant table and the 2^20-entry power table the other kernels use.
 // radix_encode_kernel (below) is the middle step of the Reed-Solomon encode of N = r * M data blocks, in place (DESIGN 3e).
 #include "mixed_radix.h"
+#include "context.h"
 #include "gf.cuh"
 
 namespace fecc {
@@ -21,16 +22,12 @@ struct RadixConsts {
     uint32_t c1[3], c2[3];     // order-3 codelet: (X + X^2)/2, (X - X^2)/2 with X = GF_Root(3) (direction applied)
 };
 
-__device__ __forceinline__ uint32_t mulc(uint32_t x, const uint32_t (&t)[3]) { return gf::canon(gf::mul(x, t[0], t[1], t[2])); }
-__device__ __forceinline__ uint32_t addm(uint32_t a, uint32_t b) { const uint32_t s = a + b; return (s < a || s >= gf::P) ? s - gf::P : s; }
-__device__ __forceinline__ uint32_t subm(uint32_t a, uint32_t b) { return a >= b ? a - b : a + (gf::P - b); }
-
 // order-3 transform of canonical residues (the arithmetic of the reference's NTT3 codelet, ntt.cpp:26-46)
 __device__ __forceinline__ void dft3(uint32_t& f0, uint32_t& f1, uint32_t& f2, const RadixConsts& C)
 {
-    const uint32_t s = addm(f1, f2), d = subm(f1, f2);
-    const uint32_t u = addm(f0, mulc(s, C.c1)), v = mulc(d, C.c2);
-    f0 = addm(f0, s); f1 = addm(u, v); f2 = subm(u, v);
+    const uint32_t s = gf::add(f1, f2), d = gf::sub(f1, f2);
+    const uint32_t u = gf::add(f0, gf::mulc(s, C.c1)), v = gf::mulc(d, C.c2);
+    f0 = gf::add(f0, s); f1 = gf::add(u, v); f2 = gf::sub(u, v);
 }
 
 // order-R transform of canonical residues in place, outputs in natural order: the order-3 codelet, or the 3 x 3 four-step of the
@@ -42,7 +39,7 @@ __device__ __forceinline__ void dft_r(uint32_t (&f)[R], const RadixConsts& C)
         dft3(f[0], f[1], f[2], C);
     } else {
         dft3(f[0], f[3], f[6], C); dft3(f[1], f[4], f[7], C); dft3(f[2], f[5], f[8], C);
-        f[4] = mulc(f[4], C.zeta[1]); f[5] = mulc(f[5], C.zeta[2]); f[7] = mulc(f[7], C.zeta[2]); f[8] = mulc(f[8], C.zeta[4]);
+        f[4] = gf::mulc(f[4], C.zeta[1]); f[5] = gf::mulc(f[5], C.zeta[2]); f[7] = gf::mulc(f[7], C.zeta[2]); f[8] = gf::mulc(f[8], C.zeta[4]);
         dft3(f[0], f[1], f[2], C); dft3(f[3], f[4], f[5], C); dft3(f[6], f[7], f[8], C);
         uint32_t g[9];
 #pragma unroll
@@ -57,7 +54,7 @@ __global__ void __launch_bounds__(256) radix_pass_kernel(const uint4* __restrict
                                                          uint32_t a_inv, uint32_t b_inv, int inverse, RadixConsts C, const uint4* __restrict__ tw)
 {
     const size_t total = (size_t)M * s4;
-    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    FOR_GRID(size_t, i, total) {
         const uint32_t k2 = (uint32_t)(i / s4), c = (uint32_t)(i - (size_t)k2 * s4);
         uint32_t f[4][R];
 #pragma unroll
@@ -70,8 +67,8 @@ __global__ void __launch_bounds__(256) radix_pass_kernel(const uint4* __restrict
             const uint4 t = tw[(size_t)em << (20 - log_m)];                    // GF_Root(M)^(+-em)
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
-                uint32_t x = gf::canon(gf::mul(f[j][n1], t.x, t.y, t.z));      // inputs are taken mod P
-                f[j][n1] = er ? mulc(x, C.zeta[er]) : x;
+                uint32_t x = gf::mulc(f[j][n1], t);      // inputs are taken mod P
+                f[j][n1] = er ? gf::mulc(x, C.zeta[er]) : x;
             }
         }
 #pragma unroll
@@ -95,12 +92,6 @@ static void fill_codelets(RadixConsts& C, uint32_t r, bool inverse)
     fill3(C.c2, gf::mulmod((uint32_t)(((uint64_t)x1 + gf::P - x2) % gf::P), inv2));
 }
 
-// grid of the grid-stride radix kernels: one thread per item, at most 16 blocks of 256 per SM
-static unsigned grid_for(size_t total, int num_sms)
-{
-    return (unsigned)((total + 255) / 256 < (size_t)num_sms * 16 ? (total + 255) / 256 : (size_t)num_sms * 16);
-}
-
 // The launchers take what api.cu has validated: r in {3, 9} (s | r for the fold), M a power of two.
 cudaError_t launch_radix_pass(const uint32_t* src, uint32_t* dst, uint32_t pitch4, uint32_t s4, uint32_t r, uint32_t M, bool inverse, const uint4* tw, int num_sms, cudaStream_t st)
 {
@@ -110,7 +101,7 @@ cudaError_t launch_radix_pass(const uint32_t* src, uint32_t* dst, uint32_t pitch
     RadixConsts C;
     fill_codelets(C, r, inverse);
     const CrtSplit ab = crt_split(r, log_m);                                   // a = M^-1 mod r, b = r^-1 mod M
-    kernel<<<grid_for((size_t)M * s4, num_sms), 256, 0, st>>>(reinterpret_cast<const uint4*>(src), reinterpret_cast<uint4*>(dst), pitch4, s4, M, log_m, ab.a, ab.b,
+    kernel<<<grid_size((size_t)M * s4, (size_t)num_sms * 16), 256, 0, st>>>(reinterpret_cast<const uint4*>(src), reinterpret_cast<uint4*>(dst), pitch4, s4, M, log_m, ab.a, ab.b,
                                                              inverse ? 1 : 0, C, tw);
     return cudaGetLastError();
 }
@@ -142,16 +133,16 @@ __device__ __forceinline__ void encode_codelets(const uint4* row, uint32_t pitch
         const uint32_t cr = (uint32_t)(((1 - 2 * n1) % R + R) % R);
         const uint32_t er = (a2 * ((k2r * cr) % R)) % R, em = (b2 * (k2 * (uint32_t)(1 - 2 * n1))) & mask;
         const uint4 t = tw[(size_t)em << sh];
-        f[0][n1] = mulc(gf::canon(gf::mul(v.x, t.x, t.y, t.z)), C.zin[er]);
-        f[1][n1] = mulc(gf::canon(gf::mul(v.y, t.x, t.y, t.z)), C.zin[er]);
-        f[2][n1] = mulc(gf::canon(gf::mul(v.z, t.x, t.y, t.z)), C.zin[er]);
-        f[3][n1] = mulc(gf::canon(gf::mul(v.w, t.x, t.y, t.z)), C.zin[er]);
+        f[0][n1] = gf::mulc(gf::mulc(v.x, t), C.zin[er]);
+        f[1][n1] = gf::mulc(gf::mulc(v.y, t), C.zin[er]);
+        f[2][n1] = gf::mulc(gf::mulc(v.z, t), C.zin[er]);
+        f[3][n1] = gf::mulc(gf::mulc(v.w, t), C.zin[er]);
     }
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
         dft_r<R>(f[j], C.inv);
 #pragma unroll
-        for (int k1 = 1; k1 < R; ++k1) f[j][k1] = mulc(f[j][k1], C.sigma[k1]);
+        for (int k1 = 1; k1 < R; ++k1) f[j][k1] = gf::mulc(f[j][k1], C.sigma[k1]);
         dft_r<R>(f[j], C.fwd);
     }
 }
@@ -162,7 +153,7 @@ __global__ void __launch_bounds__(256) radix_encode_kernel(uint4* __restrict__ x
 {
     const size_t total = (size_t)M * s4;
     const uint32_t mask = 2 * M - 1, sh = 19 - log_m;                           // GF_Root(2M)^e = tw[e << (20 - log2(2M))]
-    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    FOR_GRID(size_t, i, total) {
         const uint32_t k2 = (uint32_t)(i / s4), c = (uint32_t)(i - (size_t)k2 * s4), k2r = k2 % R;
         uint4* row = x + (size_t)R * k2 * pitch4 + c;
         uint32_t f[4][R];
@@ -175,8 +166,8 @@ __global__ void __launch_bounds__(256) radix_encode_kernel(uint4* __restrict__ x
             uint32_t o[4];
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
-                const uint32_t y = gf::canon(gf::mul(f[j][j1], t.x, t.y, t.z));
-                o[j] = er ? mulc(y, C.fwd.zeta[er]) : y;
+                const uint32_t y = gf::mulc(f[j][j1], t);
+                o[j] = er ? gf::mulc(y, C.fwd.zeta[er]) : y;
             }
             row[(size_t)j1 * pitch4] = make_uint4(o[0], o[1], o[2], o[3]);
         }
@@ -200,7 +191,7 @@ cudaError_t launch_radix_encode(uint32_t* x, uint32_t pitch4, uint32_t s4, uint3
     uint32_t log_m = 0; while ((1u << log_m) < M) ++log_m;
     EncodeConsts C;
     const CrtSplit ab = fill_encode(C, r, M, log_m);
-    kernel<<<grid_for((size_t)M * s4, num_sms), 256, 0, st>>>(reinterpret_cast<uint4*>(x), pitch4, s4, M, log_m, ab.a, ab.b, C, tw);
+    kernel<<<grid_size((size_t)M * s4, (size_t)num_sms * 16), 256, 0, st>>>(reinterpret_cast<uint4*>(x), pitch4, s4, M, log_m, ab.a, ab.b, C, tw);
     return cudaGetLastError();
 }
 
@@ -226,7 +217,7 @@ __global__ void __launch_bounds__(256) radix_fold_kernel(uint4* __restrict__ x, 
     constexpr int U = R / S;
     const size_t total = (size_t)s4 << log_t;
     const uint32_t mask = 2 * M - 1, sh = 19 - log_m;
-    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    FOR_GRID(size_t, i, total) {
         const uint32_t t = (uint32_t)(i / s4), c = (uint32_t)(i - (size_t)t * s4);
         uint32_t acc[U][4];
 #pragma unroll
@@ -237,15 +228,15 @@ __global__ void __launch_bounds__(256) radix_fold_kernel(uint4* __restrict__ x, 
             uint32_t f[4][R];
             encode_codelets<R>(row, pitch4, k2, mask, sh, a2, b2, C.e, tw, f);
 #pragma unroll
-            for (int j = 0; j < 4; ++j) acc[0][j] = addm(acc[0][j], f[j][0]);  // u = 0: J = 0, twiddle 1
+            for (int j = 0; j < 4; ++j) acc[0][j] = gf::add(acc[0][j], f[j][0]);  // u = 0: J = 0, twiddle 1
 #pragma unroll
             for (int u = 1; u < U; ++u) {
                 const uint32_t er = (C.tr[u] * k2r) % R, em = (C.tm[u] * k2) & mask;
                 const uint4 w = tw[(size_t)em << sh];
 #pragma unroll
                 for (int j = 0; j < 4; ++j) {
-                    const uint32_t y = gf::canon(gf::mul(f[j][S * u], w.x, w.y, w.z));
-                    acc[u][j] = addm(acc[u][j], er ? mulc(y, C.e.fwd.zeta[er]) : y);
+                    const uint32_t y = gf::mulc(f[j][S * u], w);
+                    acc[u][j] = gf::add(acc[u][j], er ? gf::mulc(y, C.e.fwd.zeta[er]) : y);
                 }
             }
         }
@@ -274,7 +265,7 @@ cudaError_t launch_radix_fold(uint32_t* x, uint32_t pitch4, uint32_t s4, uint32_
         C.d[u] = (uint32_t)(J / D);
     }
     const uint32_t log_t = log_m - log_fold;
-    kernel<<<grid_for((size_t)s4 << log_t, num_sms), 256, 0, st>>>(reinterpret_cast<uint4*>(x), pitch4, s4, M, log_m, log_t, 1u << log_fold, ab.a, ab.b, C, tw);
+    kernel<<<grid_size((size_t)s4 << log_t, (size_t)num_sms * 16), 256, 0, st>>>(reinterpret_cast<uint4*>(x), pitch4, s4, M, log_m, log_t, 1u << log_fold, ab.a, ab.b, C, tw);
     return cudaGetLastError();
 }
 

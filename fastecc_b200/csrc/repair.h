@@ -1,13 +1,12 @@
 // Repair of a stored stripe (N data rows + M parity rows of fastecc_b200_rs_encode_asym_mixed[_dev]): the pattern and the four
 // element-wise kernels of repair.cu; the sequence that runs them around the encode and the transforms is in api.cu.
 #pragma once
-#include <cuda_runtime.h>
-#include <stddef.h>
-#include <stdint.h>
+#include "context.h"
 
-// Everything that depends only on which blocks are lost (DESIGN 3g).  Per-row constants are Barrett triples {w, whi, wlo, 0}
-// (gf::make_tw) of canonical w.
-struct fastecc_b200_repair {
+namespace fecc {
+// Everything that depends only on which blocks are lost (DESIGN 3g), as finish_repair_kernel fills it.  Per-row constants are
+// Barrett triples {w, whi, wlo, 0} (gf::make_tw) of canonical w.
+struct RepairTables {
     size_t N = 0, M = 0, ned = 0, nep = 0;
     uint32_t* d_ed = nullptr;        // [ned] lost data rows, ascending
     uint32_t* d_ep = nullptr;        // [nep] lost parity rows, ascending
@@ -17,6 +16,11 @@ struct fastecc_b200_repair {
     uint4*    d_ck = nullptr;        // [M]   k
     uint4*    d_cd = nullptr;        // [ned] N / D[2e]
     uint4*    d_cp = nullptr;        // [nep] -2 / (M * D[2Dj' + 1])
+};
+}
+
+struct fastecc_b200_repair : fecc::RepairTables {
+    fecc::DeviceArrays mem;          // owns the arrays of the tables
 };
 
 namespace fecc {

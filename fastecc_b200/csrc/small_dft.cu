@@ -2,22 +2,16 @@
 // helpers.  One thread per 16-byte column chunk evaluates the transform by its definition (Slow_NTT,
 // ntt.cpp:451-483) -- at most 16x16 products per word -- using the same power table and GF primitives as the main kernel.
 #include "small_dft.h"
+#include "context.h"
 #include "gf.cuh"
 
 namespace fecc {
 
-__device__ __forceinline__ uint4 mul4(uint4 x, uint4 w, uint32_t z)
-{
-    x.x = gf::mul(x.x, w.x, w.y, w.z, z); x.y = gf::mul(x.y, w.x, w.y, w.z, z);
-    x.z = gf::mul(x.z, w.x, w.y, w.z, z); x.w = gf::mul(x.w, w.x, w.y, w.z, z);
-    return x;
-}
 __device__ __forceinline__ uint4 add4(uint4 a, uint4 v)
 {
     a.x = gf::addl(a.x, v.x); a.y = gf::addl(a.y, v.y); a.z = gf::addl(a.z, v.z); a.w = gf::addl(a.w, v.w);
     return a;
 }
-__device__ __forceinline__ uint4 canon4s(uint4 v) { v.x = gf::canon(v.x); v.y = gf::canon(v.y); v.z = gf::canon(v.z); v.w = gf::canon(v.w); return v; }
 
 // out[k] = sum_n in[n] * g^(z*n*k)          (n, k < N <= 16)
 __device__ __forceinline__ void dft_small(const uint4* in, uint4* out, uint32_t N, uint32_t z, const uint4* tw, uint32_t zero)
@@ -25,7 +19,7 @@ __device__ __forceinline__ void dft_small(const uint4* in, uint4* out, uint32_t 
     for (uint32_t k = 0; k < N; ++k) {
         uint4 acc = make_uint4(0, 0, 0, 0);
         for (uint32_t n = 0; n < N; ++n)
-            acc = add4(acc, mul4(in[n], tw[(z * n * k) & (gf::M - 1)], zero));
+            acc = add4(acc, gf::mul4(in[n], tw[(z * n * k) & (gf::M - 1)], zero));
         out[k] = acc;
     }
 }
@@ -43,11 +37,11 @@ __global__ void small_dft_kernel(uint32_t* data, uint32_t pitch4, uint32_t s4, u
         dft_small(x, y, N, z, tw, zero);
     } else {                                         // RS.cpp:41-63 by definition
         dft_small(x, y, N, (gf::M - 2 * q) & (gf::M - 1), tw, zero);
-        for (uint32_t m = 0; m < N; ++m) y[m] = mul4(mul4(y[m], tw[(q * m) & (gf::M - 1)], zero), invN, zero);
+        for (uint32_t m = 0; m < N; ++m) y[m] = gf::mul4(gf::mul4(y[m], tw[(q * m) & (gf::M - 1)], zero), invN, zero);
         for (uint32_t m = 0; m < N; ++m) x[m] = y[m];
         dft_small(x, y, N, 2 * q, tw, zero);
     }
-    for (uint32_t n = 0; n < N; ++n) d4[(size_t)n * pitch4 + col] = canon4s(y[n]);
+    for (uint32_t n = 0; n < N; ++n) d4[(size_t)n * pitch4 + col] = gf::canon4(y[n]);
 }
 
 cudaError_t launch_small_dft(uint32_t* data, uint32_t pitch4, uint32_t s4, uint32_t N, uint32_t z, int encode,
@@ -63,7 +57,7 @@ __global__ void repack_kernel(const uint32_t* src, size_t src_pitch, uint32_t* d
                               size_t n_rows, uint32_t size, uint32_t copy_cols, uint32_t zero_from)
 {
     const size_t total = n_rows * (size_t)copy_cols;
-    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    FOR_GRID(size_t, i, total) {
         const size_t r = i / copy_cols; const uint32_t c = (uint32_t)(i - r * copy_cols);
         dst[r * dst_pitch + c] = (c < zero_from && c < size) ? src[r * src_pitch + c] : 0u;
     }

@@ -181,26 +181,54 @@ def asym_erasures(N: int, M: int, lost_data, lost_parity):
     return sorted(rows)
 
 
-class CErasurePattern:
+class _CPattern:
+    """A pattern built on the device through the C ABI: owns the handle, which close() (or garbage collection) frees with the
+    library function named by _free."""
+    _free = None
+
+    def __init__(self):
+        import torch
+        import fastecc_b200 as fe
+        self._fe, self._lib, self._h = fe, fe.lib(), None
+        fe.init(torch.cuda.current_device())
+
+    @staticmethod
+    def _u32(values, error: str):
+        """`values` (a list, array or tensor of block or row numbers) as a contiguous uint32 array; ValueError(error) if one
+        of them is negative or does not fit 32 bits."""
+        import numpy as np
+        a = np.ascontiguousarray(np.asarray(values, dtype=np.int64).reshape(-1))
+        if a.size and (a.min() < 0 or a.max() >= (1 << 32)):
+            raise ValueError(error)
+        return a.astype(np.uint32)
+
+    def close(self):
+        if self._h:
+            getattr(self._lib, self._free)(self._h)
+        self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:            # noqa: BLE001 -- interpreter shutdown
+            pass
+
+
+class CErasurePattern(_CPattern):
     """The same decoder through the C ABI (fastecc_b200_rs_decode_pattern / _recover: csrc/decode.cu): what a C++ host uses.
     Locator, its values and derivative values are built on the device in one call; recover() is asynchronous.
     mixed=True: fastecc_b200_rs_decode_pattern_mixed, for the code words of EncodeReedSolomon_mixed / rs_encode_mixed_dev
     (n2 = 2N with N = 2^k, 3 * 2^k or 9 * 2^k, 2^k <= 2^19)."""
+    _free = "fastecc_b200_rs_decode_free"
 
     def __init__(self, n2: int, erased, mixed: bool = False):
         import ctypes
-        import numpy as np
         import torch
-        import fastecc_b200 as fe
-        self._fe, self._lib = fe, fe.lib()
-        fe.init(torch.cuda.current_device())
-        pos = np.ascontiguousarray(np.asarray(erased, dtype=np.int64))
-        if pos.size and (pos.min() < 0 or pos.max() >= (1 << 32)):
-            raise ValueError("erased: positions in [0, 2N)")
-        pos = pos.astype(np.uint32)
+        super().__init__()
+        pos = self._u32(erased, "erased: positions in [0, 2N)")
         h = ctypes.c_void_p()
         build = self._lib.fastecc_b200_rs_decode_pattern_mixed if mixed else self._lib.fastecc_b200_rs_decode_pattern
-        fe._check(build(n2, pos.ctypes.data, pos.size, torch.cuda.current_stream().cuda_stream, ctypes.byref(h)))
+        self._fe._check(build(n2, pos.ctypes.data, pos.size, torch.cuda.current_stream().cuda_stream, ctypes.byref(h)))
         self._h, self.n2, self.me = h, n2, int(pos.size)
 
     def recover(self, code):
@@ -215,69 +243,36 @@ class CErasurePattern:
                                                                     torch.cuda.current_stream(code.device).cuda_stream))
         return out[:, :S]
 
-    def close(self):
-        if self._h:
-            self._lib.fastecc_b200_rs_decode_free(self._h)
-            self._h = None
 
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:            # noqa: BLE001 -- interpreter shutdown
-            pass
-
-
-class Repair:
+class Repair(_CPattern):
     """Repair of a stored stripe in place through the C ABI (fastecc_b200_rs_repair_pattern / _repair: csrc/repair.cu, DESIGN 3g):
     the N data rows and M parity rows of EncodeReedSolomon_asym_mixed / rs_encode_asym_mixed_dev (M divides N, M = N included),
     with the blocks `lost_data` (< N) and `lost_parity` (< M) lost, at most M in all.  The pattern is built on the device once;
     repair() serves any number of stripes of any SIZE and is asynchronous on the current stream."""
+    _free = "fastecc_b200_rs_repair_free"
 
     def __init__(self, N: int, M: int, lost_data=(), lost_parity=()):
         import ctypes
-        import numpy as np
         import torch
-        import fastecc_b200 as fe
-        self._fe, self._lib, self._h = fe, fe.lib(), None
-        fe.init(torch.cuda.current_device())
-        lists = []
-        for name, lost in (("lost_data", lost_data), ("lost_parity", lost_parity)):
-            a = np.ascontiguousarray(np.asarray(lost, dtype=np.int64).reshape(-1))
-            if a.size and (a.min() < 0 or a.max() >= (1 << 32)):
-                raise ValueError("%s: block numbers in [0, 2^32)" % name)
-            lists.append(a.astype(np.uint32))
-        d, p = lists
+        super().__init__()
+        d, p = (self._u32(lost, "%s: block numbers in [0, 2^32)" % name) for name, lost in (("lost_data", lost_data), ("lost_parity", lost_parity)))
         h = ctypes.c_void_p()
-        fe._check(self._lib.fastecc_b200_rs_repair_pattern(int(N), int(M), d.ctypes.data, d.size, p.ctypes.data, p.size,
-                                                           torch.cuda.current_stream().cuda_stream, ctypes.byref(h)))
+        self._fe._check(self._lib.fastecc_b200_rs_repair_pattern(int(N), int(M), d.ctypes.data, d.size, p.ctypes.data, p.size,
+                                                                 torch.cuda.current_stream().cuda_stream, ctypes.byref(h)))
         self._h, self.N, self.M = h, int(N), int(M)
         self.lost_data, self.lost_parity = d.tolist(), p.tolist()
 
     def repair(self, data, parity):
         """data: [N, S] and parity: [M, S] int32 CUDA tensors (unit word stride), repaired in place."""
-        import torch
         if self._h is None:
             raise ValueError("the pattern was closed")
-        for t, rows, name in ((data, self.N, "data"), (parity, self.M, "parity")):
-            if not (t.is_cuda and t.dim() == 2 and t.dtype in (torch.int32, torch.uint32) and t.stride(1) == 1):
-                raise ValueError("%s: expected a 2-D CUDA int32/uint32 tensor with unit stride along the word dimension" % name)
-            if t.shape[0] != rows:
-                raise ValueError("%s has %d rows, the pattern was built for %d" % (name, t.shape[0], rows))
-        if data.shape[1] != parity.shape[1]:
-            raise ValueError("data and parity rows differ in length: %d and %d words" % (data.shape[1], parity.shape[1]))
-        self._fe._check(self._lib.fastecc_b200_rs_repair(self._h, data.data_ptr(), data.stride(0), parity.data_ptr(), parity.stride(0),
-                                                         data.shape[1], torch.cuda.current_stream(data.device).cuda_stream))
-
-    def close(self):
-        if self._h:
-            self._lib.fastecc_b200_rs_repair_free(self._h)
-        self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:            # noqa: BLE001 -- interpreter shutdown
-            pass
+        (dp, dn, S, dpitch, stream), (pp, pn, ps, ppitch, _) = self._fe._dev_args(data), self._fe._dev_args(parity)
+        for rows, want, name in ((dn, self.N, "data"), (pn, self.M, "parity")):
+            if rows != want:
+                raise ValueError("%s has %d rows, the pattern was built for %d" % (name, rows, want))
+        if S != ps:
+            raise ValueError("data and parity rows differ in length: %d and %d words" % (S, ps))
+        self._fe._check(self._lib.fastecc_b200_rs_repair(self._h, dp, dpitch, pp, ppitch, S, stream))
 
 
 def decode(code, erased, be=None):

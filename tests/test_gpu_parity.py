@@ -406,6 +406,21 @@ def test_argument_validation(fecc):
     fecc.ntt_dev(t, False)                                      # but a 2^20 NTT is legal
 
 
+def test_failed_allocation_is_not_reported_again(fecc, oracle):
+    """A host entry point whose staging buffer cannot be allocated -- 2^10 blocks of 2^31 words would take 8 TiB -- returns
+    ENOMEM (-3) before it reads a block or launches anything.  The failure is not charged to the next calls on the same thread:
+    an encode on the small-DFT path and one on the pass path right after it succeed and match the oracle."""
+    L = fecc.lib()
+    blk = np.zeros(16, dtype=np.uint32)
+    table = np.full(1 << 10, blk.ctypes.data, dtype=np.uint64)        # 1024 pointers into one small buffer, never read
+    launches = fecc.kernel_launches()
+    assert L.fastecc_b200_rs_encode(table.ctypes.data, 1 << 10, 1 << 31) == -3
+    assert fecc.kernel_launches() == launches
+    for N, S in ((16, 8), (1 << 12, 64)):
+        a = ol.fill_B(oracle, N, S)
+        assert np.array_equal(dev_encode(fecc, a), ol.o_encode(oracle, a))
+
+
 def test_device_entry_point_argument_tables(fecc):
     """One table of argument tuples per device entry point that takes a row buffer: every rule of its validation, broken on
     its own, must give FASTECC_B200_EINVAL (-1) before anything is launched (kernel_launches() does not move), and the valid

@@ -1,16 +1,12 @@
 """CPU: the repair entry points (csrc/repair.cu, api.cu) without a GPU fail with ENOINIT and compute nothing; their four
 element-wise kernels are in the library and do not spill (cuobjdump, as test_sass_evidence.py does)."""
 import ctypes
-import os
-import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-LIB = os.path.join(ROOT, "fastecc_b200", "libfastecc_b200.so")
+import sass_lib
+
 KERNELS = ("repair_load_kernel", "repair_syndrome_kernel", "repair_split_kernel", "repair_scatter_kernel")
 
 
@@ -42,18 +38,7 @@ def test_repair_without_a_gpu_is_enoinit(lib):
 
 @pytest.fixture(scope="module")
 def sass():
-    exe = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
-    if not os.path.exists(exe) or not os.path.exists(LIB):
-        pytest.skip("needs cuobjdump and the built library")
-    out = subprocess.run([exe, "-sass", LIB], capture_output=True, text=True, check=True).stdout
-    kernels, name = {}, None
-    for line in out.splitlines():
-        m = re.search(r"Function : (\S+)", line)
-        if m:
-            name = m.group(1); kernels[name] = []
-        elif name and re.match(r"\s+/\*[0-9a-f]{4,5}\*/", line):
-            kernels[name].append(line)
-    return kernels
+    return sass_lib.kernels()
 
 
 @pytest.mark.parametrize("kernel", KERNELS)

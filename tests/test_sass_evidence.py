@@ -2,33 +2,18 @@
 fastecc_b200/libfastecc_b200.so (sm_90a cubins only): the headline pass kernels take their quotient from the FP64 unit
 (I2F.F64.U32 + DFMA.RM + VIADDMNMX.U32, one each per product, and no IMAD.HI in the butterflies), load their tiles and tables
 with TMA (UTMALDG / UBLKCP + SYNCS mbarrier instructions) and do not spill."""
-import os
 import re
-import shutil
-import subprocess
 
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-LIB = os.path.join(ROOT, "fastecc_b200", "libfastecc_b200.so")
+import sass_lib
 
 
 @pytest.fixture(scope="module")
 def sass():
-    exe = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
-    if not os.path.exists(exe) or not os.path.exists(LIB):
-        pytest.skip("needs cuobjdump and the built library")
-    elf = subprocess.run([exe, "-lelf", LIB], capture_output=True, text=True, check=True).stdout
+    elf = sass_lib.dump("-lelf")
     assert "sm_90a" in elf and not re.search(r"sm_(?!90a)\d+", elf), elf
-    out = subprocess.run([exe, "-sass", LIB], capture_output=True, text=True, check=True).stdout
-    kernels, name = {}, None
-    for line in out.splitlines():
-        m = re.search(r"Function : (\S+)", line)
-        if m:
-            name = m.group(1); kernels[name] = []
-        elif name and re.match(r"\s+/\*[0-9a-f]{4,5}\*/", line):
-            kernels[name].append(line)
-    return kernels
+    return sass_lib.kernels()
 
 
 def _kernel(sass, pattern):

@@ -5,13 +5,12 @@ library's SASS, on the plans and the geometry the launcher picks for each pass (
 transforms of 2^19 and 2^20 thread by thread in that geometry against the oracle."""
 import ctypes
 import os
-import re
-import shutil
 import subprocess
 
 import pytest
 
 import oracle_lib as ol
+import sass_lib
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
@@ -20,18 +19,7 @@ LIB = os.path.join(ROOT, "fastecc_b200", "libfastecc_b200.so")
 
 @pytest.fixture(scope="module")
 def sass():
-    exe = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
-    if not os.path.exists(exe) or not os.path.exists(LIB):
-        pytest.skip("needs cuobjdump and the built library")
-    out = subprocess.run([exe, "-sass", LIB], capture_output=True, text=True, check=True).stdout
-    kernels, name = {}, None
-    for line in out.splitlines():
-        m = re.search(r"Function : (\S+)", line)
-        if m:
-            name = m.group(1); kernels[name] = []
-        elif name and re.match(r"\s+/\*[0-9a-f]{4,5}\*/", line):
-            kernels[name].append(line)
-    return kernels
+    return sass_lib.kernels()
 
 
 @pytest.mark.parametrize("lr,nxf", [(10, 1), (9, 2)])

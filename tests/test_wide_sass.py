@@ -1,31 +1,17 @@
 """CPU: the wide pass-kernel instantiations (512 threads, 128 KiB tiles; pass_threads() in ntt_tile.cuh) are in the built library,
 replace their narrow twins, load by TMA and do not spill.  cuobjdump -sass of fastecc_b200/libfastecc_b200.so."""
-import os
 import re
-import shutil
-import subprocess
 
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-LIB = os.path.join(ROOT, "fastecc_b200", "libfastecc_b200.so")
+import sass_lib
+
 WIDE = ["ntt_pass_kernelILi10ELi2ELi1ELi512E"]                       # <LR, NXF, TMA, threads>
 
 
 @pytest.fixture(scope="module")
 def sass():
-    exe = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
-    if not os.path.exists(exe) or not os.path.exists(LIB):
-        pytest.skip("needs cuobjdump and the built library")
-    out = subprocess.run([exe, "-sass", LIB], capture_output=True, text=True, check=True).stdout
-    kernels, name = {}, None
-    for line in out.splitlines():
-        m = re.search(r"Function : (\S+)", line)
-        if m:
-            name = m.group(1); kernels[name] = []
-        elif name and re.match(r"\s+/\*[0-9a-f]{4,5}\*/", line):
-            kernels[name].append(line)
-    return kernels
+    return sass_lib.kernels()
 
 
 @pytest.mark.parametrize("pattern", WIDE)
