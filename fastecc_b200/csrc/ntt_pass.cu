@@ -274,11 +274,11 @@ static cudaError_t launch_tma(const PassParams& P, const CUtensorMap& map, unsig
 }
 
 // name of the instantiation a pass is dispatched to, for the per-kernel lines of the benchmark (static storage);
-// wide instantiations carry their thread count
+// wide instantiations carry their thread count (one slot per geometry: <9,2,1> and its wide sibling share lr, nxf and tma)
 static const char* kernel_name(uint32_t lr, uint32_t nxf, uint32_t tma, int nt)
 {
-    static char names[6][3][3][40];
-    char* n = names[lr - 5][nxf][tma];
+    static char names[6][3][3][2][40];
+    char* n = names[lr - 5][nxf][tma][nt == kThreads ? 0 : 1];
     if (!n[0]) {
         if (nt == kThreads) snprintf(n, 40, "ntt_pass_kernel<%u,%u,%u>", lr, nxf, tma);
         else                snprintf(n, 40, "ntt_pass_kernel<%u,%u,%u,%d>", lr, nxf, tma, nt);
