@@ -200,7 +200,8 @@ inline std::vector<PassParams> plan_encode_asym(const Buffers& b, size_t N, size
 // One transform sharded over G GPUs (BASELINE config 4, SURVEY 8e).  Blocks are dealt cyclically: global block
 // i = l*G + g is local block l of rank g, for the data going in and for the parity coming out.  With N2 % G == 0 every
 // row set of pass A (fixed n2) and of pass D (fixed j2) is local to rank n2 % G resp. j2 % G, and every row set of
-// pass BC (fixed k1) is local to rank k1 % G after an all-to-all of whole blocks (fastecc_b200/sharded.py).  The local
+// pass BC (fixed k1) is local to rank k1 % G after an all-to-all of whole blocks (fastecc_b200/sharded.py); that needs
+// N1 % G == 0 as well, or pass BC would have N1 / G = 0 row sets on every rank and nothing would compute it.  The local
 // passes are the single-GPU ones with local strides; the only thing that knows about the sharding is the twist,
 // whose exponent t0 + set*t1 is evaluated at the GLOBAL set index set_local*G + rank.
 //   which = 0: A  on local rows n1*(N2/G) + n2'            (n2 = n2'*G + rank)
@@ -211,8 +212,8 @@ inline bool shard_supported(size_t N, uint32_t G)
     if (!is_pow2(N) || !is_pow2(G) || G < 2) return false;
     const uint32_t LN = ilog2(N);
     if (LN <= (uint32_t)kMaxLogR || LN > 19) return false;
-    const uint32_t L2 = LN - split_l1(LN, true);
-    return (1u << L2) >= G * 1u && ((1u << L2) % G) == 0;
+    const uint32_t L1 = split_l1(LN, true), L2 = LN - L1;
+    return (1u << L2) >= G * 1u && ((1u << L2) % G) == 0 && ((1u << L1) % G) == 0;
 }
 inline PassParams plan_encode_shard(const Buffers& b, size_t N, uint32_t G, uint32_t rank, int which)
 {

@@ -184,7 +184,9 @@ void fastecc_b200_rs_repair_free(fastecc_b200_repair* pattern);
  * Global block i = l*n_ranks + rank is local block l (data in, parity out).  An encode is: pass 0 on every rank,
  * all-to-all of whole blocks, pass 1, all-to-all, pass 2 -- the exchange is the caller's (fastecc_b200/sharded.py does it
  * with torch.distributed / NCCL); these are the three local passes of RS.cpp:41-63 with the sharded twists.
- * N = global number of data blocks, 2^11 .. 2^19; d_local holds N/n_ranks rows of pitch_words (16-byte aligned). */
+ * N = global number of data blocks, 2^11 .. 2^19; d_local holds N/n_ranks rows of pitch_words (16-byte aligned).  n_ranks is
+ * a power of two that divides both factors of N = N1 * N2 (fastecc_b200_shard_geometry): pass 0 and pass 2 work on N2 / n_ranks
+ * row sets per rank, pass 1 on N1 / n_ranks; other shapes fail with FASTECC_B200_EINVAL before anything is launched. */
 int fastecc_b200_rs_encode_shard_pass(uint32_t* d_local, size_t N, int n_ranks, int rank, size_t SIZE_words, size_t pitch_words,
                                       int which, void* stream);
 

@@ -510,6 +510,7 @@ def test_device_entry_point_argument_tables(fecc):
             (bad, B, 1 << 20, 2, 0, 4, 4, 0), (bad, B, 3 << 11, 2, 0, 4, 4, 0), (bad, B, 1 << 11, 64, 0, 4, 4, 0),
             (bad, B, 1 << 12, 2, 0, 0, 4, 0), (bad, B, 1 << 12, 2, 0, 8, 4, 0), (bad, B, 1 << 12, 2, 0, 4, 6, 0),
             (bad, B + 4, 1 << 12, 2, 0, 4, 4, 0), (bad, B, 1 << 19, 2, 0, 4, 1 << 16, 0),
+            (bad, B, 1 << 19, 1024, 0, 4, 4, 1),                                   # N2 = 1024 ranks, but N1 = 512 row sets for pass 1
             *[(good, B, 1 << 12, 2, r, 4, 4, w) for r in (0, 1) for w in (0, 1, 2)], (good, B, 1 << 11, 2, 0, 4, 4, 0),
         ]),
         "rs_encode_shard_pass_p2p": (L.fastecc_b200_rs_encode_shard_pass_p2p, [      # (src, peers, N, ranks, rank, SIZE, pitch, which)

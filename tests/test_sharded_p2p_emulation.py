@@ -80,3 +80,7 @@ def test_p2p_rejects_unsupported_shapes():
     p = _ptr_array([x, x])
     assert f(x.ctypes.data, p, 1 << 11, 2, 0, 4, 4, 0) == -1               # 2^11 = 64 x 32: the 32-row tiles cannot split their outputs
     assert f(x.ctypes.data, p, 1 << 12, 16, 0, 4, 4, 0) == -1              # more than 8 peers
+    g = emu.emu_rs_encode_shard_pass
+    g.argtypes = [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_int, ctypes.c_int, ctypes.c_size_t, ctypes.c_size_t, ctypes.c_int]
+    for which in (0, 1, 2):                                                 # 2^19 = 512 x 1024 over 1024 ranks: no row set of pass 1 anywhere
+        assert g(x.ctypes.data, 1 << 19, 1024, 0, 4, 4, which) == -1

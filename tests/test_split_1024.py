@@ -101,6 +101,21 @@ def test_shard_geometry_keeps_512_x_1024(G):
     assert (n1.value, n2.value) == (512, 1024)
 
 
+def test_shard_geometry_rejects_1024_ranks_at_2_to_the_19():
+    """Pass 1 of the sharded encode works on N1 / G row sets, passes 0 and 2 on N2 / G: 2^19 = 512 x 1024 cannot be dealt to 1024
+    ranks although N2 is a multiple of 1024 (every rank would get no row set of pass 1)."""
+    if not os.path.exists(LIB):
+        pytest.skip("needs the built library")
+    lib = ctypes.CDLL(LIB)
+    f = lib.fastecc_b200_shard_geometry
+    f.argtypes = [ctypes.c_size_t, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
+    f.restype = ctypes.c_int
+    ok = ctypes.c_int(-1)
+    assert f(1 << 19, 1024, None, None, ctypes.byref(ok)) == -1
+    assert ok.value == 0
+    assert f(1 << 19, 512, None, None, None) == 0
+
+
 def test_ntt_19_20_as_launched_matches_oracle(exe):
     r = subprocess.run([exe], capture_output=True, text=True, cwd=HERE, env=_env())
     assert r.returncode == 0, r.stdout[-3000:]
