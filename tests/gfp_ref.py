@@ -5,7 +5,8 @@ device (CPU tensors in the non-GPU tests, CUDA tensors beside the kernels).  Tes
   RootPowers      omega^e for omega = GF_Root(n) from a two-level table hi[e >> 12] * lo[e & 4095]
   ntt_rows        X[k] = sum_n x_n omega^(n*k mod N), omega = GF_Root(N) (forward) or its inverse (unnormalised)
   encode_rows     parity_j = f(rho^(2j+1)), rho = GF_Root(2N), f(rho^(2i)) = data_i, by the circulant form below
-  closed forms    monomial stripes for the encodes, deltas and geometric columns for the transforms
+  closed forms    monomial stripes and their 2N-row code words for the encodes and the decoders, deltas and geometric
+                  columns for the transforms
 
 Encode by definition: the Lagrange basis of the N-th roots of unity rho^(2i) evaluated at rho^(2j+1), where rho^N = -1, gives
 parity_j = (2/N) * sum_i data_i * c_((j-i) mod N) with c_d = 1 / (1 - rho^(2d+1)).  Asymmetric parity j' is row (N/M)*j'."""
@@ -129,6 +130,11 @@ def monomial_parity(N, degrees, rows=None, device="cpu", decimation=1):
     j = _rows(N // decimation, rows, device)
     m = torch.as_tensor(degrees, dtype=torch.int64, device=device)
     return powers(2 * N, device)((2 * decimation * j[:, None] + 1) * m[None, :])
+
+
+def codeword_rows(N, degrees, rows=None, device="cpu"):
+    """Rows of the 2N-row code word of the monomial stripe: row x = rho^(x*m_c) (data i is row 2i, parity j is row 2j + 1)."""
+    return powers(2 * N, device)(_rows(2 * N, rows, device)[:, None] * torch.as_tensor(degrees, dtype=torch.int64, device=device)[None, :])
 
 
 def delta_ntt_columns(N, positions, rows=None, device="cpu", inverse=False):
