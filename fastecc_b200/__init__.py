@@ -70,6 +70,7 @@ def lib() -> ctypes.CDLL:
         L.fastecc_b200_rs_repair_pattern.argtypes = [sz, sz, vp, sz, vp, sz, vp, ctypes.POINTER(vp)]; L.fastecc_b200_rs_repair_pattern.restype = ci
         L.fastecc_b200_rs_repair.argtypes = [vp, vp, sz, vp, sz, sz, vp]; L.fastecc_b200_rs_repair.restype = ci
         L.fastecc_b200_rs_repair_free.argtypes = [vp]; L.fastecc_b200_rs_repair_free.restype = None
+        L.fastecc_b200_rs_update.argtypes = [vp, sz, sz, vp, sz, sz, vp, sz, vp, sz, sz, vp]; L.fastecc_b200_rs_update.restype = ci
         L.fastecc_b200_rs_encode_shard_pass.argtypes = [vp, sz, ci, ci, sz, sz, ci, vp]; L.fastecc_b200_rs_encode_shard_pass.restype = ci
         L.fastecc_b200_rs_encode_shard_pass_p2p.argtypes = [vp, vp, sz, ci, ci, sz, sz, ci, vp]; L.fastecc_b200_rs_encode_shard_pass_p2p.restype = ci
         L.fastecc_b200_ntt_shard_pass_p2p.argtypes = [vp, vp, sz, ci, ci, sz, sz, ci, ci, vp]; L.fastecc_b200_ntt_shard_pass_p2p.restype = ci
@@ -272,6 +273,22 @@ def rs_repair_dev(data, parity, lost_data, lost_parity) -> None:
         r.repair(data, parity)
     finally:
         r.close()
+
+
+def rs_update_dev(data, parity, changed, new) -> None:
+    """Update a stored stripe in place (fastecc_b200_rs_update, DESIGN 3h): data = the N data rows, parity = the M parity rows
+    of rs_encode_asym_mixed_dev (int32 CUDA tensors, 16-byte aligned rows with pitches that are multiples of 4 words); changed =
+    ascending distinct block numbers below N; row i of `new` is the new content of data block changed[i].  The changed data rows
+    receive their canonical new blocks and the parity becomes the encode of the updated data; the stored parity must be the
+    encode of the stored data.  Asynchronous on the current stream."""
+    from .decoder import _CPattern
+    (dp, N, S, dpitch, stream), (pp, M, ps, ppitch, _), (nptr, k, ns, npitch, _) = _dev_args(data), _dev_args(parity), _dev_args(new)
+    idx = _CPattern._u32(changed, "changed: block numbers in [0, 2^32)")
+    if k != idx.size:
+        raise ValueError("new has %d rows for %d changed blocks" % (k, idx.size))
+    if not S == ps == ns:
+        raise ValueError("data, parity and new rows differ in length: %d, %d and %d words" % (S, ps, ns))
+    _check(lib().fastecc_b200_rs_update(dp, dpitch, N, pp, ppitch, M, idx.ctypes.data, idx.size, nptr, npitch, S, stream))
 
 
 def bytes_to_gfp_dev(raw, words=None):

@@ -7,6 +7,8 @@
 #include "elementwise.h"
 #include "mixed_radix.h"
 #include "repair.h"
+#include "update.h"
+#include "locator.h"
 #include <cuda_runtime.h>
 #include <cstdio>
 #include <cstdarg>
@@ -48,10 +50,10 @@ struct DevBuf {
 // Stage tables of one pass: built once, on the stream of the first call that needs them.  `ready` is recorded behind the
 // build; a call on any other stream waits for it (a no-op once the build has finished).
 struct TableSlot { DevBuf buf; cudaEvent_t ready = nullptr; cudaStream_t built_on = nullptr; };
-enum Kind { kNtt, kEncode, kEncodeAsym, kShard, kShardP2P, kNttShardP2P };
+enum Kind { kNtt, kEncode, kEncodeAsym, kShard, kShardP2P, kNttShardP2P, kUpdate };
 struct TableKey {                        // what the stage tables of a plan depend on
     int kind, inverse, n_ranks, rank;
-    int sub;                             // which pass of a sharded plan, or log2(N / M) of an asymmetric encode
+    int sub;                             // which pass of a sharded plan, log2(N / M) of an asymmetric encode, r of kUpdate's N = r * 2^k
     int log_n;
     bool operator<(const TableKey& o) const
     { return std::tie(kind, inverse, n_ranks, rank, sub, log_n) < std::tie(o.kind, o.inverse, o.n_ranks, o.rank, o.sub, o.log_n); }
@@ -98,7 +100,10 @@ struct Context {
     SharedBuf scratch;   // Y buffer of the two-pass NTT and of the asymmetric encode
     SharedBuf packed;    // repacked copy for unaligned device layouts
     SharedBuf mixed;     // destination of the order-3 / order-9 step of the N = 3 * 2^k, 9 * 2^k transforms
-    SharedBuf repair;    // workspace of fastecc_b200_rs_repair: N + M rows of one column chunk
+    SharedBuf repair;    // workspace of fastecc_b200_rs_repair: N + M rows of one column chunk; and of fastecc_b200_rs_update
+    struct HostList { uint32_t* p = nullptr; size_t cap = 0; cudaEvent_t copied = nullptr; };
+    std::vector<HostList> lists;         // page-locked copies of fastecc_b200_rs_update's changed lists (used under repair's lease)
+    size_t next_list = 0;                // the one to wait for next once there are kMaxLists
     DevBuf staging;      // device copy for the host (T**) entry points (serialised by g_host_mu)
     std::map<TableKey, std::vector<TableSlot>> tables;   // one slot per pass of the plan
     bool pin_caller = false;                          // fastecc_b200_pin_host_buffers()
@@ -169,8 +174,28 @@ void pin_caller_array(Context* c, void* base, size_t bytes)
     else clear_cuda_error();
 }
 
-// Stage tables of `plan` under cache key `key`: built on first use (a block enters the cache only once it is allocated and
-// its build launched), then attached to the passes.
+// The table block of slot `sl` (caller holds g_mu): built on first use by the one launch `build(buffer)` on `st` (a block enters
+// the cache only once it is allocated and its build launched); a call on another stream waits for the build.
+template <class Build>
+int use_table(TableSlot& sl, size_t bytes, cudaStream_t st, Build build)
+{
+    if (!sl.buf.p) {
+        DevBuf nb;
+        cudaEvent_t ev = nullptr;
+        cudaError_t e = nb.reserve(bytes);
+        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
+        if (e == cudaSuccess) e = build((uint4*)nb.p);
+        if (e == cudaSuccess) e = cudaEventRecord(ev, st);
+        if (e != cudaSuccess) { nb.release(); if (ev) cudaEventDestroy(ev); CUDA_TRY(e); }
+        g_launches++;
+        sl.buf = nb; sl.ready = ev; sl.built_on = st;
+    } else if (sl.built_on != st) {
+        CUDA_TRY(cudaStreamWaitEvent(st, sl.ready, 0));
+    }
+    return 0;
+}
+
+// Stage tables of `plan` under cache key `key`, attached to the passes.
 int attach_tables(Context* c, const TableKey& key, std::vector<PassParams>& plan, cudaStream_t st)
 {
     std::lock_guard<std::mutex> lk(g_mu);
@@ -178,19 +203,7 @@ int attach_tables(Context* c, const TableKey& key, std::vector<PassParams>& plan
     slots.resize(plan.size());
     for (size_t i = 0; i < plan.size(); ++i) {
         TableSlot& sl = slots[i];
-        if (!sl.buf.p) {
-            DevBuf nb;
-            cudaEvent_t ev = nullptr;
-            cudaError_t e = nb.reserve(table_bytes(plan[i]));
-            if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
-            if (e == cudaSuccess) e = launch_build_tables(plan[i], (uint4*)nb.p, st);
-            if (e == cudaSuccess) e = cudaEventRecord(ev, st);
-            if (e != cudaSuccess) { nb.release(); if (ev) cudaEventDestroy(ev); CUDA_TRY(e); }
-            g_launches++;
-            sl.buf = nb; sl.ready = ev; sl.built_on = st;
-        } else if (sl.built_on != st) {
-            CUDA_TRY(cudaStreamWaitEvent(st, sl.ready, 0));
-        }
+        if (int rc = use_table(sl, table_bytes(plan[i]), st, [&](uint4* t) { return launch_build_tables(plan[i], t, st); })) return rc;
         plan[i].tables = (const uint4*)sl.buf.p;
         plan[i].table_set_stride = table_sets(plan[i]) > 1 ? (plan[i].nxf << plan[i].log_r) : 0u;
     }
@@ -465,14 +478,127 @@ int repair(Context* c, const fastecc_b200_repair* R, uint32_t* data, size_t dpit
     uint32_t* x = ws.ptr();
     for (size_t c0 = 0; c0 < size; c0 += w) {
         const size_t cols = size - c0 < w ? size - c0 : w;
-        CUDA_TRY(launch_repair_load(R, data, dpitch, c0, x, w, cols, c->num_sms, st)); g_launches++;
+        CUDA_TRY(launch_repair_load(N, R->d_lost, data, dpitch, c0, x, w, cols, c->num_sms, st)); g_launches++;
         if (int rc = encode(c, x, N, M, cols, w, st)) return rc;
-        CUDA_TRY(launch_repair_syndrome(R, parity, ppitch, c0, size, x, w, cols, c->num_sms, st)); g_launches++;
+        CUDA_TRY(launch_repair_syndrome(M, R->d_cs, parity, ppitch, c0, size, x, w, cols, c->num_sms, st)); g_launches++;
         if (M > 1) { if (int rc = ntt(c, x, M, cols, w, true, st)) return rc; }
         CUDA_TRY(launch_repair_split(R, x, w, cols, c->num_sms, st)); g_launches++;
         if (R->ned && N > 1) { if (int rc = ntt(c, x, N, cols, w, false, st)) return rc; }
         if (R->nep && M > 1) { if (int rc = ntt(c, x + N * w, M, cols, w, false, st)) return rc; }
         CUDA_TRY(launch_repair_scatter(R, data, dpitch, parity, ppitch, c0, size, x, w, cols, c->num_sms, st)); g_launches++;
+    }
+    return 0;
+}
+
+// Whether a device buffer of `rows` rows (the first SIZE words of each) shares a word with another.
+bool rows_overlap(const void* a, size_t a_rows, size_t a_pitch, const void* b, size_t b_rows, size_t b_pitch, size_t size)
+{
+    const uintptr_t a0 = (uintptr_t)a, a1 = a0 + ((a_rows - 1) * a_pitch + size) * 4;
+    const uintptr_t b0 = (uintptr_t)b, b1 = b0 + ((b_rows - 1) * b_pitch + size) * 4;
+    return a0 < b1 && b0 < a1;
+}
+
+// The table T of fastecc_b200_rs_update at order N (update.h), built on first use and cached like the stage tables.
+int update_table(Context* c, size_t N, cudaStream_t st, const uint4** T)
+{
+    const Order o = split_order(N);
+    std::lock_guard<std::mutex> lk(g_mu);
+    std::vector<TableSlot>& slots = c->tables[{kUpdate, 0, 0, 0, (int)o.r, (int)o.log2_m}];
+    slots.resize(1);
+    if (int rc = use_table(slots[0], N * sizeof(uint4), st, [&](uint4* t) { return launch_update_table(t, N, st); })) return rc;
+    *T = (const uint4*)slots[0].buf.p;
+    return 0;
+}
+
+// The caller's host list of k changed rows into d_idx without waiting for the stream: a pageable source could make
+// cudaMemcpyAsync synchronise, so the list goes through one of the context's page-locked buffers, one whose last copy has run.
+// While fewer than kMaxLists exist, a new one is added when none is free and large enough (one that is new because the list
+// outgrew them all is at least twice the largest); after that the buffers are taken in turn, waiting for the copy out of the
+// next one, so a caller that queues many updates behind long work holds at most kMaxLists of them.  Freeing page-locked memory
+// could synchronise the device, so a buffer is only replaced when it is too small.  The caller holds repair's lease.
+constexpr size_t kMaxLists = 8;
+int upload_list(Context* c, const uint32_t* changed, size_t k, uint32_t* d_idx, cudaStream_t st)
+{
+    Context::HostList* h = nullptr;
+    size_t largest = 0;
+    for (Context::HostList& b : c->lists) {
+        largest = b.cap > largest ? b.cap : largest;
+        if (h || b.cap < k) continue;
+        const cudaError_t e = cudaEventQuery(b.copied);
+        if (e == cudaSuccess) h = &b;
+        else clear_cuda_error();                                     // cudaErrorNotReady: still in flight
+    }
+    size_t cap = k <= largest ? k : k > 2 * largest ? k : 2 * largest;
+    if (cap < 4096) cap = 4096;
+    if (!h && c->lists.size() >= kMaxLists) {
+        h = &c->lists[c->next_list];
+        c->next_list = (c->next_list + 1) % kMaxLists;
+        CUDA_TRY(cudaEventSynchronize(h->copied));
+        if (h->cap < k) {
+            cudaFreeHost(h->p); h->p = nullptr; h->cap = 0;
+            CUDA_TRY(cudaHostAlloc((void**)&h->p, cap * sizeof(uint32_t), cudaHostAllocDefault));
+            h->cap = cap;
+        }
+    }
+    if (!h) {
+        Context::HostList b;
+        b.cap = cap;
+        CUDA_TRY(cudaEventCreateWithFlags(&b.copied, cudaEventDisableTiming));
+        if (cudaError_t e = cudaHostAlloc((void**)&b.p, b.cap * sizeof(uint32_t), cudaHostAllocDefault)) { cudaEventDestroy(b.copied); CUDA_TRY(e); }
+        c->lists.push_back(b);
+        h = &c->lists.back();
+    }
+    memcpy(h->p, changed, k * sizeof(uint32_t));
+    CUDA_TRY(cudaMemcpyAsync(d_idx, h->p, k * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaEventRecord(h->copied, st));
+    return 0;
+}
+
+// The path of an update of k of N data blocks with M parity blocks of SIZE words (DESIGN 3h), in units of one product per
+// 16-byte lane at full occupancy.  The direct path costs k times the lanes of update_parity_kernel's grid (32 parity rows x 32
+// chunks per CTA, padding included: ceil32(M) * ceil32(s4)) plus kUpdateRowLanes per changed row, the part of a row's cost that
+// does not shrink with the grid (a grid too small to fill the GPU runs each row at the latency of one CTA).  The re-encode costs
+// about eight passes over the N data rows whatever k, kUpdateDirect * N * s4, plus kUpdateFixed for its launches and short-row
+// passes.  The direct path also needs its k delta rows within repair's 4 GiB bound.  The three constants are fitted to where the
+// measured curves cross on the H100 at the eleven points of tools/sweep.py --update.
+size_t update_lanes(size_t M, size_t s4) { return (M + 31) / 32 * 32 * ((s4 + 31) / 32 * 32); }
+#if defined(FECC_UPDATE_PATH)            // experiment switch (DESIGN 13): 1 = always direct, 2 = always re-encode (tools/sweep.py --update)
+bool update_direct(size_t, size_t, size_t, size_t) { return FECC_UPDATE_PATH == 1; }
+#else
+constexpr size_t kUpdateDirect = 20, kUpdateRowLanes = 400000, kUpdateFixed = 50000000;
+bool update_direct(size_t N, size_t M, size_t k, size_t size)
+{
+    const size_t s4 = (size + 3) / 4;
+    if (k * s4 * 16 > kMaxRepairBytes) return false;
+    return k * (update_lanes(M, s4) + kUpdateRowLanes) <= kUpdateDirect * N * s4 + kUpdateFixed;
+}
+#endif
+
+// The update of one stripe (DESIGN 3h), on the repair workspace: either the k delta rows (direct) or N rows of one column chunk
+// (re-encode), from the start of the buffer so that every row keeps the allocation's alignment, then the k indices.  Direct:
+// delta, then the parity update.  Re-encode: the new rows in place, then per column chunk repair's load with no row lost, the
+// encode of api.cu, and the store of all M parity rows.
+int update(Context* c, uint32_t* data, size_t dpitch, size_t N, uint32_t* parity, size_t ppitch, size_t M, const uint32_t* changed, size_t k,
+           const uint32_t* nw, size_t npitch, size_t size, cudaStream_t st)
+{
+    const bool direct = update_direct(N, M, k, size);
+    const size_t s4 = (size + 3) / 4, w = direct ? 0 : repair_chunk_words(N, M, size), rows_words = direct ? k * s4 * 4 : N * w;
+    const uint4* T = nullptr;
+    if (direct) { if (int rc = update_table(c, N, st, &T)) return rc; }
+    Lease ws(&c->repair, st);
+    CUDA_TRY(ws.acquire((rows_words + k) * sizeof(uint32_t)));
+    uint32_t *x = ws.ptr(), *idx = x + rows_words;
+    if (int rc = upload_list(c, changed, k, idx, st)) return rc;
+    CUDA_TRY(launch_update_delta(data, dpitch, nw, npitch, direct ? (uint4*)x : nullptr, idx, k, size, c->num_sms, st)); g_launches++;
+    if (direct) {
+        CUDA_TRY(launch_update_parity(parity, ppitch, M, (const uint4*)x, idx, k, T, N, size, st)); g_launches++;
+        return 0;
+    }
+    for (size_t c0 = 0; c0 < size; c0 += w) {
+        const size_t cols = size - c0 < w ? size - c0 : w;
+        CUDA_TRY(launch_repair_load(N, nullptr, data, dpitch, c0, x, w, cols, c->num_sms, st)); g_launches++;
+        if (int rc = encode(c, x, N, M, cols, w, st)) return rc;
+        CUDA_TRY(launch_repair_syndrome(M, nullptr, parity, ppitch, c0, size, x, w, cols, c->num_sms, st)); g_launches++;
     }
     return 0;
 }
@@ -519,6 +645,7 @@ void fastecc_b200_shutdown(void)
     cudaDeviceSynchronize();
     g_ctx->scratch.destroy(); g_ctx->packed.destroy(); g_ctx->mixed.destroy(); g_ctx->repair.destroy(); g_ctx->staging.release();
     for (auto& r : g_ctx->registered) cudaHostUnregister(r.first);
+    for (auto& l : g_ctx->lists) { cudaFreeHost(l.p); cudaEventDestroy(l.copied); }
     for (auto& kv : g_ctx->tables) for (auto& sl : kv.second) { sl.buf.release(); if (sl.ready) cudaEventDestroy(sl.ready); }
     if (g_ctx->d_tw) cudaFree(g_ctx->d_tw);
     if (g_ctx->stream) cudaStreamDestroy(g_ctx->stream);
@@ -732,11 +859,28 @@ int fastecc_b200_rs_repair(const fastecc_b200_repair* R, uint32_t* d_data, size_
     if (!R) return fail(FASTECC_B200_EINVAL, "%s: null pattern", who);
     if (int rc = check_rows(d_data, R->N, size, data_pitch, true, who)) return rc;
     if (int rc = check_rows(d_parity, R->M, size, parity_pitch, true, who)) return rc;
-    const uintptr_t d0 = (uintptr_t)d_data, d1 = d0 + ((R->N - 1) * data_pitch + size) * 4;
-    const uintptr_t p0 = (uintptr_t)d_parity, p1 = p0 + ((R->M - 1) * parity_pitch + size) * 4;
-    if (d0 < p1 && p0 < d1) return fail(FASTECC_B200_EINVAL, "%s: the data and parity buffers overlap", who);
+    if (rows_overlap(d_data, R->N, data_pitch, d_parity, R->M, parity_pitch, size)) return fail(FASTECC_B200_EINVAL, "%s: the data and parity buffers overlap", who);
     if (R->ned + R->nep == 0) return 0;
     return repair(c, R, d_data, data_pitch, d_parity, parity_pitch, size, (cudaStream_t)stream);
+}
+
+int fastecc_b200_rs_update(uint32_t* d_data, size_t data_pitch, size_t N, uint32_t* d_parity, size_t parity_pitch, size_t M,
+                           const uint32_t* changed, size_t n_changed, const uint32_t* d_new, size_t new_pitch, size_t size, void* stream)
+{
+    const char* who = "fastecc_b200_rs_update";
+    Context* c = ctx(who);
+    if (!c) return FASTECC_B200_ENOINIT;
+    if (int rc = check_order(N, M, size, padded_pitch(size), FASTECC_B200_MAX_LOG_N_ENCODE, true, who)) return rc;
+    if (int rc = check_rows(d_data, N, size, data_pitch, true, who)) return rc;
+    if (int rc = check_rows(d_parity, M, size, parity_pitch, true, who)) return rc;
+    if (n_changed && !changed) return fail(FASTECC_B200_EINVAL, "%s: null list of changed blocks", who);
+    if (!ascending_below(changed, n_changed, N)) return fail(FASTECC_B200_EINVAL, "%s: changed data blocks must be ascending, distinct and below N=%zu", who, N);
+    if (rows_overlap(d_data, N, data_pitch, d_parity, M, parity_pitch, size)) return fail(FASTECC_B200_EINVAL, "%s: the data and parity buffers overlap", who);
+    if (!n_changed) return 0;
+    if (int rc = check_rows(d_new, n_changed, size, new_pitch, true, who)) return rc;
+    if (rows_overlap(d_new, n_changed, new_pitch, d_data, N, data_pitch, size) || rows_overlap(d_new, n_changed, new_pitch, d_parity, M, parity_pitch, size))
+        return fail(FASTECC_B200_EINVAL, "%s: the new blocks overlap the data or the parity buffer", who);
+    return update(c, d_data, data_pitch, N, d_parity, parity_pitch, M, changed, n_changed, d_new, new_pitch, size, (cudaStream_t)stream);
 }
 
 int fastecc_b200_pin_host_buffers(int enable)

@@ -52,6 +52,17 @@ inline unsigned grid_size(size_t n, size_t cap)
     return (unsigned)(blocks < cap ? (blocks ? blocks : 1) : cap);
 }
 
+#if defined(__CUDACC__)
+// Words [w, w + 4) of `row`, of which only those below `size` are written: 16-byte stores, scalar ones in a partial last group.
+__device__ __forceinline__ void store_row(uint32_t* row, size_t w, const uint4& v, size_t size)
+{
+    if (w + 4 <= size) { *reinterpret_cast<uint4*>(row + w) = v; return; }
+    if (w < size) row[w] = v.x;
+    if (w + 1 < size) row[w + 1] = v.y;
+    if (w + 2 < size) row[w + 2] = v.z;
+}
+#endif
+
 } // namespace fecc
 
 #define CUDA_TRY(expr) do { const cudaError_t e_ = (expr); if (e_ != cudaSuccess) return ::fecc::cuda_fail(e_, #expr); } while (0)

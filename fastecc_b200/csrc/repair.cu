@@ -20,39 +20,32 @@ using namespace fecc;
 constexpr uint32_t P = gf::P;
 
 // ---- the four element-wise kernels: flat over (row, 16-byte chunk), per-row constants as Barrett triples --------------------
-// words [w, w + 4) of `row`, of which only those below `size` are written (the last chunk of a row may be partial)
-__device__ __forceinline__ void store_row(uint32_t* row, size_t w, const uint4& v, size_t size)
-{
-    if (w + 4 <= size) { *reinterpret_cast<uint4*>(row + w) = v; return; }
-    if (w < size) row[w] = v.x;
-    if (w + 1 < size) row[w + 1] = v.y;
-    if (w + 2 < size) row[w + 2] = v.z;
-}
-
+// lost == nullptr: no row is lost (the re-encode of fastecc_b200_rs_update)
 __global__ void __launch_bounds__(256) repair_load_kernel(const uint32_t* __restrict__ data, size_t dpitch, size_t c0, uint4* __restrict__ ws, size_t wpitch4,
                                                           uint32_t s4, uint32_t n, const uint8_t* __restrict__ lost)
 {
     FOR_GRID(uint32_t, i, n) {
         const uint32_t row = i / s4, c = i - row * s4;
         uint4 v = make_uint4(0, 0, 0, 0);
-        if (!lost[row]) v = gf::canon4(__ldg(reinterpret_cast<const uint4*>(data + row * dpitch + c0) + c));
+        if (!lost || !lost[row]) v = gf::canon4(__ldg(reinterpret_cast<const uint4*>(data + row * dpitch + c0) + c));
         ws[row * wpitch4 + c] = v;
     }
 }
 
+// cs == nullptr: every parity row takes G and the workspace is left as it is (the re-encode of fastecc_b200_rs_update)
 __global__ void __launch_bounds__(256) repair_syndrome_kernel(uint32_t* __restrict__ parity, size_t ppitch, size_t c0, size_t size, uint4* __restrict__ ws,
                                                               size_t wpitch4, uint32_t s4, uint32_t n, const uint4* __restrict__ cs)
 {
     const uint32_t zero = gf::opaque_zero();
     FOR_GRID(uint32_t, i, n) {
         const uint32_t row = i / s4, c = i - row * s4;
-        const uint4 k = __ldg(cs + row);
+        const uint4 k = cs ? __ldg(cs + row) : make_uint4(0, 0, 0, 0);
         uint4* g = ws + row * wpitch4 + c;
         uint32_t* prow = parity + row * ppitch;
         const uint4 G = *g;
         if (k.x == 0) {                                          // lost: the parity of the zeroed data goes in place, u = 0
             store_row(prow, c0 + 4 * (size_t)c, G, size);
-            *g = make_uint4(0, 0, 0, 0);
+            if (cs) *g = make_uint4(0, 0, 0, 0);
         } else {
             const uint4 v = gf::canon4(*reinterpret_cast<const uint4*>(prow + c0 + 4 * (size_t)c));
             *g = gf::canon4(gf::mul4(make_uint4(gf::sub(v.x, G.x), gf::sub(v.y, G.y), gf::sub(v.z, G.z), gf::sub(v.w, G.w)), k, zero));
@@ -157,19 +150,19 @@ int build_repair(fastecc_b200_repair* R, const uint32_t* lost_data, const uint32
 
 namespace fecc {
 
-cudaError_t launch_repair_load(const fastecc_b200_repair* R, const uint32_t* data, size_t dpitch, size_t c0, uint32_t* ws, size_t wpitch,
+cudaError_t launch_repair_load(size_t N, const uint8_t* lost, const uint32_t* data, size_t dpitch, size_t c0, uint32_t* ws, size_t wpitch,
                                size_t cols, int num_sms, cudaStream_t st)
 {
-    const uint32_t s4 = (uint32_t)((cols + 3) / 4), n = (uint32_t)(R->N * s4);
-    repair_load_kernel<<<grid_size(n, (size_t)num_sms * 16), 256, 0, st>>>(data, dpitch, c0, reinterpret_cast<uint4*>(ws), wpitch / 4, s4, n, R->d_lost);
+    const uint32_t s4 = (uint32_t)((cols + 3) / 4), n = (uint32_t)(N * s4);
+    repair_load_kernel<<<grid_size(n, (size_t)num_sms * 16), 256, 0, st>>>(data, dpitch, c0, reinterpret_cast<uint4*>(ws), wpitch / 4, s4, n, lost);
     return cudaGetLastError();
 }
 
-cudaError_t launch_repair_syndrome(const fastecc_b200_repair* R, uint32_t* parity, size_t ppitch, size_t c0, size_t size, uint32_t* ws, size_t wpitch,
+cudaError_t launch_repair_syndrome(size_t M, const uint4* cs, uint32_t* parity, size_t ppitch, size_t c0, size_t size, uint32_t* ws, size_t wpitch,
                                    size_t cols, int num_sms, cudaStream_t st)
 {
-    const uint32_t s4 = (uint32_t)((cols + 3) / 4), n = (uint32_t)(R->M * s4);
-    repair_syndrome_kernel<<<grid_size(n, (size_t)num_sms * 16), 256, 0, st>>>(parity, ppitch, c0, size, reinterpret_cast<uint4*>(ws), wpitch / 4, s4, n, R->d_cs);
+    const uint32_t s4 = (uint32_t)((cols + 3) / 4), n = (uint32_t)(M * s4);
+    repair_syndrome_kernel<<<grid_size(n, (size_t)num_sms * 16), 256, 0, st>>>(parity, ppitch, c0, size, reinterpret_cast<uint4*>(ws), wpitch / 4, s4, n, cs);
     return cudaGetLastError();
 }
 

@@ -27,11 +27,12 @@ namespace fecc {
 // All four work on a column chunk of `cols` words starting at word c0 (a multiple of 4) of the caller's rows, against a workspace
 // of pitch wpitch words (rows [0, N) data side, rows [N, N + M) the k * P_k rows).  The caller's rows are written at words
 // [c0, min(c0 + cols, size)) only.
-// load: ws[i] = data[i] mod P, or 0 on a lost data row, i < N
-cudaError_t launch_repair_load(const fastecc_b200_repair* R, const uint32_t* data, size_t dpitch, size_t c0, uint32_t* ws, size_t wpitch,
+// load: ws[i] = data[i] mod P, or 0 on a lost data row (lost[i] != 0), i < N; lost = nullptr: no row is lost
+cudaError_t launch_repair_load(size_t N, const uint8_t* lost, const uint32_t* data, size_t dpitch, size_t c0, uint32_t* ws, size_t wpitch,
                                size_t cols, int num_sms, cudaStream_t st);
-// syndrome: j' < M surviving: ws[j'] = (parity[j'] - ws[j']) * cs[j'];  lost: parity[j'] = ws[j'] (= G_j'), ws[j'] = 0
-cudaError_t launch_repair_syndrome(const fastecc_b200_repair* R, uint32_t* parity, size_t ppitch, size_t c0, size_t size, uint32_t* ws, size_t wpitch,
+// syndrome: j' < M surviving: ws[j'] = (parity[j'] - ws[j']) * cs[j'];  lost (cs[j'] = 0): parity[j'] = ws[j'] (= G_j'), ws[j'] = 0;
+// cs = nullptr: parity[j'] = ws[j'] for every j' < M, the workspace untouched (the store of a re-encode)
+cudaError_t launch_repair_syndrome(size_t M, const uint4* cs, uint32_t* parity, size_t ppitch, size_t c0, size_t size, uint32_t* ws, size_t wpitch,
                                    size_t cols, int num_sms, cudaStream_t st);
 // split: k < M: ws[N + k] = k * ws[k] (if parity was lost), ws[k] *= cr[k];  ws[M .. N) = 0 (if data was lost)
 cudaError_t launch_repair_split(const fastecc_b200_repair* R, uint32_t* ws, size_t wpitch, size_t cols, int num_sms, cudaStream_t st);

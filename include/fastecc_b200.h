@@ -180,6 +180,29 @@ int  fastecc_b200_rs_repair(const fastecc_b200_repair* pattern, uint32_t* d_data
                             uint32_t* d_parity, size_t parity_pitch_words, size_t SIZE_words, void* stream);
 void fastecc_b200_rs_repair_free(fastecc_b200_repair* pattern);
 
+/* ---- update of a stored stripe, in place -------------------------------------------------------------------------------
+ * The write of a stored stripe: n_changed of its N data blocks get new content, and the M parity rows are brought up to date
+ * without re-encoding the stripe from scratch.  The stripe is that of fastecc_b200_rs_repair: d_data = N rows
+ * (data_pitch_words apart) and d_parity = M rows (parity_pitch_words apart) as fastecc_b200_rs_encode_asym_mixed[_dev] leaves them,
+ * for any (N, M) that fastecc_b200_rs_encode_asym_mixed_dev accepts.  changed: HOST array, ascending, distinct, below N; row i of
+ * d_new (new_pitch_words apart) is the new content of data block changed[i].
+ * PRECONDITION: the stored parity is the encode of the stored data.  On a stripe where it is not, the result is unspecified
+ * (the update adds the change to the parity; it does not re-derive the parity from the data).
+ * On return data rows changed[i] hold the canonical new blocks and the parity rows equal fastecc_b200_rs_encode_asym_mixed_dev of
+ * the updated data, bit for bit.  Nothing else is written: no other data row, no pad word beyond SIZE in any buffer, never d_new.
+ * Every input word, old or new, data or parity, is taken mod P.  All three buffers 16-byte aligned with pitches that are
+ * multiples of 4 words, none overlapping another.  Validated in full before anything is allocated or launched.  Asynchronous on
+ * the stream, which it does not synchronise; `changed` may be freed as soon as the call returns.  n_changed == 0 returns 0 and
+ * launches nothing.
+ * The library picks one of two paths from (N, M, n_changed, SIZE) (DESIGN 3h): for few changed blocks, the change times a table
+ * of N coefficients (16 bytes each, built on the device at the first update of an N and kept by the context) is added to the
+ * parity rows, reading only the changed rows and the parity (workspace: the n_changed delta rows, at most 4 GiB); for many, the
+ * new rows are written and the whole stripe is re-encoded into the parity, in column chunks as fastecc_b200_rs_repair runs
+ * (same workspace, same 4 GiB bound).  The host side keeps at most 8 page-locked copies of changed lists in flight; a call
+ * beyond that waits for the oldest copy to have run. */
+int fastecc_b200_rs_update(uint32_t* d_data, size_t data_pitch_words, size_t N, uint32_t* d_parity, size_t parity_pitch_words, size_t M,
+                           const uint32_t* changed, size_t n_changed, const uint32_t* d_new, size_t new_pitch_words, size_t SIZE_words, void* stream);
+
 /* ---- one transform sharded over several GPUs (one process per GPU; BASELINE config 4) ---------------------------
  * Global block i = l*n_ranks + rank is local block l (data in, parity out).  An encode is: pass 0 on every rank,
  * all-to-all of whole blocks, pass 1, all-to-all, pass 2 -- the exchange is the caller's (fastecc_b200/sharded.py does it

@@ -250,9 +250,93 @@ def repair_sweep(S):
         torch.cuda.empty_cache()
 
 
+def update_sweep():
+    """Update of k data blocks of a stored stripe (fastecc_b200_rs_update, DESIGN 3h) on each of its two paths.  The library picks
+    the path itself, so builds of it that differ only in -DFECC_UPDATE_PATH=1 (always direct) and =2 (always re-encode), and a
+    third that is always direct with the quotient of its products on the FP64 unit (-DFECC_UPDATE_MUL_H, gf::mul_h), are compiled
+    into a temporary directory and loaded side by side.  CUDA events around `reps` back-to-back calls, the builds alternated twice
+    (the lower figures); at k = 1 also an in-place torch op over the same parity tensor (parity.add_(1), one read and one write of
+    the same bytes).  k runs over powers of 4 and 100 (a count whose index list is not a multiple of 64 words) until the direct
+    path takes more than twice the re-encode.  Each line names the card and its power limit, read in the same run."""
+    import ctypes
+    import shutil
+    import subprocess
+    import tempfile
+    from bench import gpu_identity
+    from fastecc_b200 import build as b
+    card = gpu_identity(torch.cuda.current_device())
+    tmp = tempfile.mkdtemp(prefix="fastecc_update_")
+    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
+    builds = []
+    for name, flags in (("direct", ["-DFECC_UPDATE_PATH=1"]), ("reencode", ["-DFECC_UPDATE_PATH=2"]), ("direct_mul_h", ["-DFECC_UPDATE_PATH=1", "-DFECC_UPDATE_MUL_H"])):
+        out = os.path.join(tmp, "libfastecc_b200_%s.so" % name)
+        cmd = [nvcc] + b.NVCC_FLAGS + flags + ["-o", out] + [os.path.join(b.CSRC, s) for s in b.SOURCES]
+        builds.append((name, subprocess.Popen(cmd), out))
+    libs = {}
+    for name, proc, out in builds:
+        if proc.wait() != 0:
+            raise RuntimeError("nvcc failed building %s" % out)
+        L = ctypes.CDLL(out)
+        sz, vp = ctypes.c_size_t, ctypes.c_void_p
+        L.fastecc_b200_rs_update.argtypes = [vp, sz, sz, vp, sz, sz, vp, sz, vp, sz, sz, vp]
+        L.fastecc_b200_rs_encode_asym_mixed_dev.argtypes = [vp, sz, sz, sz, sz, vp]
+        L.fastecc_b200_last_error.restype = ctypes.c_char_p
+        if L.fastecc_b200_init(0):
+            raise RuntimeError(L.fastecc_b200_last_error().decode())
+        libs[name] = L
+
+    def call(L, rc):
+        if rc:
+            raise RuntimeError(L.fastecc_b200_last_error().decode())
+
+    rng = np.random.default_rng(1)
+    points = [(1 << 19, m, 1024) for m in (1 << 19, 1 << 18, 1 << 15, 1 << 13, 1 << 11, 1 << 8, 1 << 4, 1)]
+    points += [(3 << 19, 1 << 19, 1024), (9 << 18, 1 << 18, 1024), (1 << 19, 1 << 15, 16)]
+    for N, M, S in points:
+        stream = torch.cuda.current_stream().cuda_stream
+        data = (torch.arange(N * S, device="cuda", dtype=torch.int64) % P).to(torch.int32).view(N, S)
+        buf = data.clone()
+        call(libs["reencode"], libs["reencode"].fastecc_b200_rs_encode_asym_mixed_dev(buf.data_ptr(), N, M, S, S, stream))
+        parity = buf[:M].clone()
+        del buf
+        torch.cuda.empty_cache()
+        ks = sorted({4 ** i for i in range(12) if 4 ** i <= N} | ({100} if N >= 100 else set()))
+        for k in ks:
+            changed = np.sort(rng.choice(N, size=k, replace=False)).astype(np.uint32)
+            new = torch.randint(0, P, (k, S), device="cuda", dtype=torch.int64).to(torch.int32)
+            reps = 5
+
+            def run(L):
+                return lambda: call(L, L.fastecc_b200_rs_update(data.data_ptr(), S, N, parity.data_ptr(), S, M, changed.ctypes.data, k,
+                                                                 new.data_ptr(), S, S, stream))
+            runs = {name: [] for name in libs}
+            for _ in range(2):
+                for name, L in libs.items():
+                    runs[name].append(timed(run(L), reps))
+            line = {"op": "update", "N": N, "M": M, "k": k, "block_bytes": 4 * S, "reps": reps}
+            for name in libs:
+                line[name + "_ms"] = round(min(runs[name]), 4)
+                line[name + "_runs"] = [round(v, 4) for v in runs[name]]
+            line.update(faster="direct" if min(runs["direct"]) < min(runs["reencode"]) else "reencode", gpu=card["name"], power_limit_w=card["power_limit_w"])
+            if k == 1:                                        # (the parity is stale afterwards; no timing depends on its content)
+                line["torch_add_on_parity_ms"] = round(timed(lambda: parity.add_(1), 10), 4)
+            print(json.dumps(line), flush=True)
+            del new
+            if min(runs["direct"]) > 2 * min(runs["reencode"]):
+                break
+        del data, parity
+        torch.cuda.empty_cache()
+    for L in libs.values():
+        L.fastecc_b200_shutdown()
+    shutil.rmtree(tmp, ignore_errors=True)
+
+
 if __name__ == "__main__":
     if "--repair" in sys.argv:                                # only the repair lines
         fe.init(0)
         repair_sweep(1024)
+        sys.exit(0)
+    if "--update" in sys.argv:                                # only the update lines
+        update_sweep()
         sys.exit(0)
     sys.exit(main())
