@@ -71,6 +71,7 @@ def lib() -> ctypes.CDLL:
         L.fastecc_b200_rs_repair.argtypes = [vp, vp, sz, vp, sz, sz, vp]; L.fastecc_b200_rs_repair.restype = ci
         L.fastecc_b200_rs_repair_free.argtypes = [vp]; L.fastecc_b200_rs_repair_free.restype = None
         L.fastecc_b200_rs_update.argtypes = [vp, sz, sz, vp, sz, sz, vp, sz, vp, sz, sz, vp]; L.fastecc_b200_rs_update.restype = ci
+        L.fastecc_b200_rs_scrub.argtypes = [vp, sz, sz, vp, sz, sz, sz, sz, ctypes.c_uint64, vp, vp, vp, vp, vp, vp]; L.fastecc_b200_rs_scrub.restype = ci
         L.fastecc_b200_rs_encode_shard_pass.argtypes = [vp, sz, ci, ci, sz, sz, ci, vp]; L.fastecc_b200_rs_encode_shard_pass.restype = ci
         L.fastecc_b200_rs_encode_shard_pass_p2p.argtypes = [vp, vp, sz, ci, ci, sz, sz, ci, vp]; L.fastecc_b200_rs_encode_shard_pass_p2p.restype = ci
         L.fastecc_b200_ntt_shard_pass_p2p.argtypes = [vp, vp, sz, ci, ci, sz, sz, ci, ci, vp]; L.fastecc_b200_ntt_shard_pass_p2p.restype = ci
@@ -289,6 +290,27 @@ def rs_update_dev(data, parity, changed, new) -> None:
     if not S == ps == ns:
         raise ValueError("data, parity and new rows differ in length: %d, %d and %d words" % (S, ps, ns))
     _check(lib().fastecc_b200_rs_update(dp, dpitch, N, pp, ppitch, M, idx.ctypes.data, idx.size, nptr, npitch, S, stream))
+
+
+SCRUB_CLEAN, SCRUB_LOCATED, SCRUB_DETECTED = 0, 1, 2
+
+
+def rs_scrub_dev(data, parity, max_bad: int = 0, seed: int = 0):
+    """Scrub a stored stripe (fastecc_b200_rs_scrub, DESIGN 3i): data = the N data rows, parity = the M parity rows of
+    rs_encode_asym_mixed_dev (int32 CUDA tensors, 16-byte aligned rows with pitches that are multiples of 4 words), read only.
+    Returns (status, bad_data, bad_parity): SCRUB_CLEAN if the parity is the encode of the data; SCRUB_LOCATED with the ascending
+    lists of corrupted data and parity blocks (at most max_bad in all, ready for rs_repair_dev); SCRUB_DETECTED if corrupted but
+    not located within max_bad (0 = detect only; at most min(M // 2, 4096)).  `seed` picks the fold weights (the header states
+    them).  Synchronises the current stream."""
+    (dp, N, S, dpitch, stream), (pp, M, ps, ppitch, _) = _dev_args(data), _dev_args(parity)
+    if S != ps:
+        raise ValueError("data and parity rows differ in length: %d and %d words" % (S, ps))
+    cap = max(int(max_bad), 1)
+    bd, bp = np.zeros(cap, dtype=np.uint32), np.zeros(cap, dtype=np.uint32)
+    status, nd, npar = ctypes.c_int(-1), ctypes.c_size_t(0), ctypes.c_size_t(0)
+    _check(lib().fastecc_b200_rs_scrub(dp, dpitch, N, pp, ppitch, M, S, int(max_bad), int(seed) & ((1 << 64) - 1), stream, ctypes.byref(status),
+                                       bd.ctypes.data, ctypes.byref(nd), bp.ctypes.data, ctypes.byref(npar)))
+    return status.value, [int(x) for x in bd[:nd.value]], [int(x) for x in bp[:npar.value]]
 
 
 def bytes_to_gfp_dev(raw, words=None):

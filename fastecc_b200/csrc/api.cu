@@ -8,8 +8,10 @@
 #include "mixed_radix.h"
 #include "repair.h"
 #include "update.h"
+#include "scrub.h"
 #include "locator.h"
 #include <cuda_runtime.h>
+#include <algorithm>
 #include <cstdio>
 #include <cstdarg>
 #include <cstring>
@@ -100,7 +102,7 @@ struct Context {
     SharedBuf scratch;   // Y buffer of the two-pass NTT and of the asymmetric encode
     SharedBuf packed;    // repacked copy for unaligned device layouts
     SharedBuf mixed;     // destination of the order-3 / order-9 step of the N = 3 * 2^k, 9 * 2^k transforms
-    SharedBuf repair;    // workspace of fastecc_b200_rs_repair: N + M rows of one column chunk; and of fastecc_b200_rs_update
+    SharedBuf repair;    // workspace of fastecc_b200_rs_repair: N + M rows of one column chunk; and of fastecc_b200_rs_update and _scrub
     struct HostList { uint32_t* p = nullptr; size_t cap = 0; cudaEvent_t copied = nullptr; };
     std::vector<HostList> lists;         // page-locked copies of fastecc_b200_rs_update's changed lists (used under repair's lease)
     size_t next_list = 0;                // the one to wait for next once there are kMaxLists
@@ -603,6 +605,68 @@ int update(Context* c, uint32_t* data, size_t dpitch, size_t N, uint32_t* parity
     return 0;
 }
 
+// The scrub of one stripe (DESIGN 3i) on the repair workspace: N + M single-column rows of 4 words (the two folds in words 0
+// and 1), then four flag words {syndrome nonzero, check failed, data roots, parity roots} and the two root lists of `cap` words.
+// Fold, reduce, encode, syndromes, inverse order-M transform; one sync for the flag and S^_0 .. S^_(2 max_bad - 1) of fold 0;
+// Berlekamp-Massey on the host; then C's order-M transform (parity roots), the product with s, the inverse transform and the
+// check of [L, M), and the order-N transform of C_k rho^-k (data roots); a second sync for the flags and the lists.  The caller's
+// outputs are written only once every runtime call has succeeded, so an error return leaves them as they were.
+constexpr size_t kMaxScrubBad = FASTECC_B200_SCRUB_MAX_BAD;
+int scrub(Context* c, const uint32_t* data, size_t dpitch, size_t N, const uint32_t* parity, size_t ppitch, size_t M, size_t size, size_t max_bad,
+          uint64_t seed, cudaStream_t st, int* status, uint32_t* bad_data, size_t* n_bad_data, uint32_t* bad_parity, size_t* n_bad_parity)
+{
+    const size_t rows = N + M, cap = max_bad ? max_bad : 1;
+    Lease ws(&c->repair, st);
+    CUDA_TRY(ws.acquire((rows * 4 + 4 + 2 * cap) * sizeof(uint32_t)));
+    uint32_t *x = ws.ptr(), *flags = x + rows * 4, *list_d = flags + 4, *list_p = list_d + cap;
+    CUDA_TRY(cudaMemsetAsync(x, 0, (rows * 4 + 4) * sizeof(uint32_t), st));
+    CUDA_TRY(launch_scrub_fold(data, dpitch, N, parity, ppitch, M, size, seed, x, c->num_sms, st)); g_launches++;
+    CUDA_TRY(launch_scrub_reduce(x, rows, st)); g_launches++;
+    TRY_RC(encode(c, x, N, M, 2, 4, st));
+    CUDA_TRY(launch_scrub_syndrome(x, N, M, flags, st)); g_launches++;
+    if (max_bad) TRY_RC(ntt(c, x, M, 2, 4, true, st));                         // max_bad >= 1: M >= 2
+    uint32_t h[4];
+    std::vector<uint32_t> S(2 * max_bad);
+    CUDA_TRY(cudaMemcpyAsync(h, flags, sizeof h, cudaMemcpyDeviceToHost, st));
+    if (max_bad) CUDA_TRY(cudaMemcpy2DAsync(S.data(), 4, x, 16, 4, S.size(), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    auto result = [&](int s) { *status = s; *n_bad_data = *n_bad_parity = 0; return 0; };
+    if (!h[0]) return result(FASTECC_B200_SCRUB_CLEAN);
+    if (!max_bad) return result(FASTECC_B200_SCRUB_DETECTED);
+    std::vector<uint32_t> C;
+    const size_t L = berlekamp_massey(S, C);
+    if (L > max_bad || C.size() != L + 1) return result(FASTECC_B200_SCRUB_DETECTED);
+    // the parity points zeta^j: C(zeta^j), then M * (C * S^ mod z^M - 1) = INTT_M(C(zeta^j) * s_j) in both folds
+    CUDA_TRY(cudaMemsetAsync(x, 0, M * 16, st));
+    CUDA_TRY(cudaMemcpy2DAsync(x, 16, C.data(), 4, 4, L + 1, cudaMemcpyHostToDevice, st));
+    TRY_RC(ntt(c, x, M, 2, 4, false, st));
+    CUDA_TRY(launch_scrub_roots(x, M, list_p, flags + 3, cap, st)); g_launches++;
+    CUDA_TRY(launch_scrub_product(x, N, M, st)); g_launches++;
+    TRY_RC(ntt(c, x, M, 2, 4, true, st));
+    CUDA_TRY(launch_scrub_check(x, L, M, flags + 1, st)); g_launches++;
+    // the data points omega^i: C(rho^-1 omega^i) = NTT_N(C_k rho^-k)[i]
+    const uint32_t rho_inv = gf::inv(gf::root((uint32_t)(2 * N)));
+    std::vector<uint32_t> T(L + 1);
+    for (size_t k = 0, r = 1; k <= L; ++k, r = gf::mulmod((uint32_t)r, rho_inv)) T[k] = gf::mulmod(C[k], (uint32_t)r);
+    CUDA_TRY(cudaMemsetAsync(x, 0, N * 16, st));
+    CUDA_TRY(cudaMemcpy2DAsync(x, 16, T.data(), 4, 4, L + 1, cudaMemcpyHostToDevice, st));
+    TRY_RC(ntt(c, x, N, 2, 4, false, st));                                     // N >= M >= 2
+    CUDA_TRY(launch_scrub_roots(x, N, list_d, flags + 2, cap, st)); g_launches++;
+    std::vector<uint32_t> ld(cap), lp(cap);
+    CUDA_TRY(cudaMemcpyAsync(h, flags, sizeof h, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(ld.data(), list_d, cap * 4, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(lp.data(), list_p, cap * 4, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    if (h[1] || (size_t)h[2] + h[3] != L) return result(FASTECC_B200_SCRUB_DETECTED);   // C fails the check, or a root is no stripe point
+    std::sort(ld.begin(), ld.begin() + h[2]);
+    std::sort(lp.begin(), lp.begin() + h[3]);
+    std::copy(ld.begin(), ld.begin() + h[2], bad_data);
+    std::copy(lp.begin(), lp.begin() + h[3], bad_parity);
+    *n_bad_data = h[2]; *n_bad_parity = h[3];
+    *status = FASTECC_B200_SCRUB_LOCATED;
+    return 0;
+}
+
 } // namespace
 
 namespace fecc {
@@ -881,6 +945,24 @@ int fastecc_b200_rs_update(uint32_t* d_data, size_t data_pitch, size_t N, uint32
     if (rows_overlap(d_new, n_changed, new_pitch, d_data, N, data_pitch, size) || rows_overlap(d_new, n_changed, new_pitch, d_parity, M, parity_pitch, size))
         return fail(FASTECC_B200_EINVAL, "%s: the new blocks overlap the data or the parity buffer", who);
     return update(c, d_data, data_pitch, N, d_parity, parity_pitch, M, changed, n_changed, d_new, new_pitch, size, (cudaStream_t)stream);
+}
+
+int fastecc_b200_rs_scrub(const uint32_t* d_data, size_t data_pitch, size_t N, const uint32_t* d_parity, size_t parity_pitch, size_t M, size_t size,
+                          size_t max_bad, uint64_t seed, void* stream, int* status, uint32_t* bad_data, size_t* n_bad_data, uint32_t* bad_parity,
+                          size_t* n_bad_parity)
+{
+    const char* who = "fastecc_b200_rs_scrub";
+    Context* c = ctx(who);
+    if (!c) return FASTECC_B200_ENOINIT;
+    if (!status || !n_bad_data || !n_bad_parity) return fail(FASTECC_B200_EINVAL, "%s: null status or count output", who);
+    if (int rc = check_order(N, M, size, padded_pitch(size), FASTECC_B200_MAX_LOG_N_ENCODE, true, who)) return rc;
+    if (int rc = check_rows(d_data, N, size, data_pitch, true, who)) return rc;
+    if (int rc = check_rows(d_parity, M, size, parity_pitch, true, who)) return rc;
+    if (max_bad > M / 2 || max_bad > kMaxScrubBad)
+        return fail(FASTECC_B200_EINVAL, "%s: max_bad=%zu must be at most min(M / 2, %zu) = %zu", who, max_bad, kMaxScrubBad, M / 2 < kMaxScrubBad ? M / 2 : kMaxScrubBad);
+    if (max_bad && (!bad_data || !bad_parity)) return fail(FASTECC_B200_EINVAL, "%s: null list of bad blocks", who);
+    return scrub(c, d_data, data_pitch, N, d_parity, parity_pitch, M, size, max_bad, seed, (cudaStream_t)stream, status, bad_data, n_bad_data, bad_parity,
+                 n_bad_parity);
 }
 
 int fastecc_b200_pin_host_buffers(int enable)

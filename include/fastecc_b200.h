@@ -187,7 +187,8 @@ void fastecc_b200_rs_repair_free(fastecc_b200_repair* pattern);
  * for any (N, M) that fastecc_b200_rs_encode_asym_mixed_dev accepts.  changed: HOST array, ascending, distinct, below N; row i of
  * d_new (new_pitch_words apart) is the new content of data block changed[i].
  * PRECONDITION: the stored parity is the encode of the stored data.  On a stripe where it is not, the result is unspecified
- * (the update adds the change to the parity; it does not re-derive the parity from the data).
+ * (the update adds the change to the parity; it does not re-derive the parity from the data).  fastecc_b200_rs_scrub below checks
+ * it, and locates the blocks that break it.
  * On return data rows changed[i] hold the canonical new blocks and the parity rows equal fastecc_b200_rs_encode_asym_mixed_dev of
  * the updated data, bit for bit.  Nothing else is written: no other data row, no pad word beyond SIZE in any buffer, never d_new.
  * Every input word, old or new, data or parity, is taken mod P.  All three buffers 16-byte aligned with pitches that are
@@ -202,6 +203,38 @@ void fastecc_b200_rs_repair_free(fastecc_b200_repair* pattern);
  * beyond that waits for the oldest copy to have run. */
 int fastecc_b200_rs_update(uint32_t* d_data, size_t data_pitch_words, size_t N, uint32_t* d_parity, size_t parity_pitch_words, size_t M,
                            const uint32_t* changed, size_t n_changed, const uint32_t* d_new, size_t new_pitch_words, size_t SIZE_words, void* stream);
+
+/* ---- scrub of a stored stripe: detect silent corruption, locate the corrupted blocks ------------------------------------
+ * The stripe of fastecc_b200_rs_repair (N data rows, M parity rows, any (N, M) that fastecc_b200_rs_encode_asym_mixed_dev accepts,
+ * both buffers 16-byte aligned with pitches that are multiples of 4 words; they may overlap, since nothing is written).  The
+ * code has minimum distance M + 1, so from the stripe alone the call tells whether the parity is the encode of the data, and
+ * locates up to max_bad corrupted blocks at unknown positions, data and parity alike (DESIGN 3i).
+ *   max_bad:  0 = detect only (the only choice at M = 1); else 1 <= max_bad <= min(M / 2, FASTECC_B200_SCRUB_MAX_BAD) (the
+ *             locator is found by Berlekamp-Massey on the host, O(max_bad^2)).
+ *   seed:     the two folds of the columns use the weights r_f,c (fold f in {0, 1}, column c < SIZE):
+ *                 z = seed + (2c + f + 1) * 0x9E3779B97F4A7C15                       (mod 2^64)
+ *                 z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9;  z = (z ^ (z >> 27)) * 0x94D049BB133111EB;  z ^= z >> 31
+ *                 r_f,c = z mod P
+ *             i.e. the (2c + f + 1)-th output of splitmix64 started at `seed`.  Row m folds to sum_c r_f,c * row_m[c] mod P.  The
+ *             same seed gives the same result; a scrub that must not be predictable by whoever writes the data takes a fresh one.
+ *   Out:      *status = FASTECC_B200_SCRUB_*; bad_data / bad_parity: HOST arrays of capacity max_bad (may be NULL when max_bad = 0)
+ *             receive the located blocks, ascending (ready for fastecc_b200_rs_repair_pattern), *n_bad_data / *n_bad_parity their
+ *             counts (0 unless LOCATED).  None of the outputs is written when the call returns an error.
+ * Guarantees, with t corrupted blocks (blocks with any word of their SIZE that differs mod P from the encode of the stored data,
+ * parity blocks counted against the data as stored), each up to a probability of P^-2 over the folds' weights (P^-1 per fold):
+ *   t = 0 -> CLEAN;  1 <= t <= max_bad -> LOCATED with exactly the corrupted blocks;  max_bad < t <= M - max_bad -> DETECTED;
+ *   1 <= t <= M -> never CLEAN.  Beyond M - max_bad the result may be LOCATED with a wrong set, as for every bounded-distance
+ *   decoder.  Words are taken mod P (a raw word >= P congruent to the stored value is not corruption), pad words beyond SIZE are
+ *   never read into a sum.
+ * Validated in full before anything is allocated or launched.  Synchronises the stream (the host needs the syndromes).  Device
+ * memory: (N + M) * 16 bytes of the context's repair workspace plus the encode's and the transforms' buffers for one column. */
+#define FASTECC_B200_SCRUB_CLEAN     0   /* the parity is the encode of the data                  */
+#define FASTECC_B200_SCRUB_LOCATED   1   /* bad_data / bad_parity list every corrupted block      */
+#define FASTECC_B200_SCRUB_DETECTED  2   /* corrupted, not located within max_bad                 */
+#define FASTECC_B200_SCRUB_MAX_BAD   4096
+int fastecc_b200_rs_scrub(const uint32_t* d_data, size_t data_pitch_words, size_t N, const uint32_t* d_parity, size_t parity_pitch_words, size_t M,
+                          size_t SIZE_words, size_t max_bad, uint64_t seed, void* stream, int* status,
+                          uint32_t* bad_data, size_t* n_bad_data, uint32_t* bad_parity, size_t* n_bad_parity);
 
 /* ---- one transform sharded over several GPUs (one process per GPU; BASELINE config 4) ---------------------------
  * Global block i = l*n_ranks + rank is local block l (data in, parity out).  An encode is: pass 0 on every rank,

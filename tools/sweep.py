@@ -4,7 +4,7 @@ encode at N = 2^7 .. 2^19 and forward NTT at N = 2^10 .. 2^20, 4096-byte blocks,
 calls.  Arrays below ~100 MB stay in the 126 MB L2 between calls (marked); the small orders are launch-latency bound.
 Then recoding, decoding, the asymmetric encode, the encode of 3 * 2^k / 9 * 2^k blocks (`encode_mixed`, DESIGN 3e) and
 their encode into fewer parity blocks (`encode_asym_mixed`, DESIGN 3f; `--asym-mixed`: only these).  `--repair`: only the repair
-of a stored stripe against the 2N-row decoder (DESIGN 3g).
+of a stored stripe against the 2N-row decoder (DESIGN 3g); `--update`, `--scrub`: only the update (3h) or the scrub (3i) lines.
 Prints one JSON line per point."""
 import json
 import os
@@ -331,7 +331,105 @@ def update_sweep():
     shutil.rmtree(tmp, ignore_errors=True)
 
 
+def scrub_sweep():
+    """Scrub of a stored stripe (fastecc_b200_rs_scrub, DESIGN 3i), shipped build against one whose fold takes the products'
+    quotient on the FP64 unit (-DFECC_SCRUB_MUL_H, gf::mul_h), compiled into a temporary directory and loaded side by side.  The
+    whole call: CUDA events around `reps` back-to-back calls (each synchronises the stream itself).  The fold kernel alone: its
+    device time in a torch.profiler trace of the same calls.  The two builds alternated twice (the lower figures).  For the fold,
+    the fraction of its memory floor ((N + M) * SIZE * 4 bytes at the data sheet's 3.35 TB/s) and of update's measured product
+    rate (2 (N + M) SIZE products at 1.7e12 per second, DESIGN 3h).  Beside it, today's detect-only route: copy the data into a
+    preallocated buffer, rs_encode_asym_mixed_dev, torch.equal against the parity.  t corrupted blocks, half data and half
+    parity, max_bad = min(M / 2, 4096); the host's Berlekamp-Massey time is scrub - (its time at t = 0) roughly.  Each line
+    names the card and its power limit, read in the same run."""
+    import ctypes
+    import shutil
+    import subprocess
+    import tempfile
+    from torch.profiler import ProfilerActivity, profile
+    from bench import gpu_identity
+    from fastecc_b200 import build as b
+    fe.init(0)
+    card = gpu_identity(torch.cuda.current_device())
+    tmp = tempfile.mkdtemp(prefix="fastecc_scrub_")
+    out = os.path.join(tmp, "libfastecc_b200_mul_h.so")
+    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
+    subprocess.run([nvcc] + b.NVCC_FLAGS + ["-DFECC_SCRUB_MUL_H", "-o", out] + [os.path.join(b.CSRC, src) for src in b.SOURCES], check=True)
+    libs = {"mul": fe.lib(), "mul_h": ctypes.CDLL(out)}
+    sz, vp = ctypes.c_size_t, ctypes.c_void_p
+    for L in libs.values():
+        L.fastecc_b200_rs_scrub.argtypes = [vp, sz, sz, vp, sz, sz, sz, sz, ctypes.c_uint64, vp, vp, vp, vp, vp, vp]
+        L.fastecc_b200_last_error.restype = ctypes.c_char_p
+    if libs["mul_h"].fastecc_b200_init(0):
+        raise RuntimeError(libs["mul_h"].fastecc_b200_last_error().decode())
+
+    def scrub(L, data, parity, max_bad):
+        cap = max(max_bad, 1)
+        bd, bp = np.zeros(cap, dtype=np.uint32), np.zeros(cap, dtype=np.uint32)
+        st, nd, npar = ctypes.c_int(), ctypes.c_size_t(), ctypes.c_size_t()
+        rc = L.fastecc_b200_rs_scrub(data.data_ptr(), data.stride(0), data.shape[0], parity.data_ptr(), parity.stride(0), parity.shape[0], data.shape[1],
+                                     max_bad, 7, torch.cuda.current_stream().cuda_stream, ctypes.byref(st), bd.ctypes.data, ctypes.byref(nd),
+                                     bp.ctypes.data, ctypes.byref(npar))
+        if rc:
+            raise RuntimeError(L.fastecc_b200_last_error().decode())
+        return st.value
+
+    def fold_ms(L, data, parity, max_bad, reps):
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(reps):
+                scrub(L, data, parity, max_bad)
+            torch.cuda.synchronize()
+        us = [e.device_time_total for e in prof.key_averages() if "scrub_fold_kernel" in e.key]
+        return us[0] / 1000 / reps if us else float("nan")
+
+    S, reps = 1024, 5
+    points = [(1 << 19, m) for m in (1 << 19, 1 << 18, 1 << 15, 1 << 13, 16, 1)] + [(3 << 19, 1 << 19), (9 << 18, 1 << 18)]
+    rng = np.random.default_rng(1)
+    for N, M in points:
+        data = (torch.arange(N * S, device="cuda", dtype=torch.int64) * 2654435761 % P).to(torch.int32).view(N, S)
+        buf = data.clone()
+        fe.rs_encode_asym_mixed_dev(buf, M)
+        parity = buf[:M].clone()
+        torch.cuda.synchronize()
+        max_bad = min(M // 2, 4096)
+
+        def reencode():
+            buf.copy_(data)
+            fe.rs_encode_asym_mixed_dev(buf, M)
+            return torch.equal(buf[:M], parity)
+        reencode_ms = timed(reencode, 3)
+        for t in sorted({0, 1, 16, max_bad} & set(range(0, max_bad + 1))):
+            nd = t // 2
+            bd = np.sort(rng.choice(N, size=nd, replace=False)); bp = np.sort(rng.choice(M, size=t - nd, replace=False))
+            keep_d, keep_p = data[bd].clone(), parity[bp].clone()
+            data[bd] ^= 1; parity[bp] ^= 2
+            statuses = {name: scrub(L, data, parity, max_bad) for name, L in libs.items()}
+            ms = {name: [] for name in libs}
+            fold = {name: [] for name in libs}
+            for _ in range(2):
+                for name, L in libs.items():
+                    ms[name].append(timed(lambda: scrub(L, data, parity, max_bad), reps if t < 4096 else 2))
+                    fold[name].append(fold_ms(L, data, parity, max_bad, reps if t < 4096 else 2))
+            rows = N + M
+            mem_ms, prod_ms = rows * S * 4 / 3.35e12 * 1e3, 2 * rows * S / 1.7e12 * 1e3
+            line = {"op": "scrub", "N": N, "M": M, "t": t, "max_bad": max_bad, "block_bytes": 4 * S, "status": statuses["mul"],
+                    "status_mul_h": statuses["mul_h"], "fold_memory_floor_ms": round(mem_ms, 4), "fold_product_ms_at_1.7e12": round(prod_ms, 4),
+                    "reencode_compare_ms": round(reencode_ms, 4), "gpu": card["name"], "power_limit_w": card["power_limit_w"]}
+            for name in libs:
+                f = min(fold[name])
+                line.update({"scrub_ms_" + name: round(min(ms[name]), 4), "fold_ms_" + name: round(f, 4),
+                             "fold_of_memory_floor_" + name: round(mem_ms / f, 3), "fold_of_product_rate_" + name: round(prod_ms / f, 3)})
+            print(json.dumps(line), flush=True)
+            data[bd] = keep_d; parity[bp] = keep_p
+        del data, buf, parity
+        torch.cuda.empty_cache()
+    libs["mul_h"].fastecc_b200_shutdown()
+    shutil.rmtree(tmp, ignore_errors=True)
+
+
 if __name__ == "__main__":
+    if "--scrub" in sys.argv:                                 # only the scrub lines
+        scrub_sweep()
+        sys.exit(0)
     if "--repair" in sys.argv:                                # only the repair lines
         fe.init(0)
         repair_sweep(1024)
