@@ -72,6 +72,7 @@ def lib() -> ctypes.CDLL:
         L.fastecc_b200_rs_repair_free.argtypes = [vp]; L.fastecc_b200_rs_repair_free.restype = None
         L.fastecc_b200_rs_update.argtypes = [vp, sz, sz, vp, sz, sz, vp, sz, vp, sz, sz, vp]; L.fastecc_b200_rs_update.restype = ci
         L.fastecc_b200_rs_scrub.argtypes = [vp, sz, sz, vp, sz, sz, sz, sz, ctypes.c_uint64, vp, vp, vp, vp, vp, vp]; L.fastecc_b200_rs_scrub.restype = ci
+        L.fastecc_b200_rs_scrub_degraded.argtypes = [vp, vp, sz, vp, sz, sz, sz, ctypes.c_uint64, vp, vp, vp, vp, vp, vp]; L.fastecc_b200_rs_scrub_degraded.restype = ci
         L.fastecc_b200_rs_encode_shard_pass.argtypes = [vp, sz, ci, ci, sz, sz, ci, vp]; L.fastecc_b200_rs_encode_shard_pass.restype = ci
         L.fastecc_b200_rs_encode_shard_pass_p2p.argtypes = [vp, vp, sz, ci, ci, sz, sz, ci, vp]; L.fastecc_b200_rs_encode_shard_pass_p2p.restype = ci
         L.fastecc_b200_ntt_shard_pass_p2p.argtypes = [vp, vp, sz, ci, ci, sz, sz, ci, ci, vp]; L.fastecc_b200_ntt_shard_pass_p2p.restype = ci
@@ -311,6 +312,19 @@ def rs_scrub_dev(data, parity, max_bad: int = 0, seed: int = 0):
     _check(lib().fastecc_b200_rs_scrub(dp, dpitch, N, pp, ppitch, M, S, int(max_bad), int(seed) & ((1 << 64) - 1), stream, ctypes.byref(status),
                                        bd.ctypes.data, ctypes.byref(nd), bp.ctypes.data, ctypes.byref(npar)))
     return status.value, [int(x) for x in bd[:nd.value]], [int(x) for x in bp[:npar.value]]
+
+
+def rs_scrub_degraded_dev(data, parity, lost_data, lost_parity, max_bad: int = 0, seed: int = 0):
+    """Scrub a degraded stripe (fastecc_b200_rs_scrub_degraded, DESIGN 3j): rs_scrub_dev with the blocks lost_data / lost_parity
+    known lost (fewer than M in all; their rows are never read).  The survivors are checked: (status, bad_data, bad_parity) with
+    the corrupted survivors when LOCATED (max_bad at most min((M - f) // 2, 4096), f lost blocks).  Repair with lost + located
+    blocks afterwards.  One-shot form of decoder.Repair(...).scrub (which builds the pattern once)."""
+    from .decoder import Repair
+    r = Repair(data.shape[0], parity.shape[0], lost_data, lost_parity)
+    try:
+        return r.scrub(data, parity, max_bad, seed)
+    finally:
+        r.close()
 
 
 def bytes_to_gfp_dev(raw, words=None):

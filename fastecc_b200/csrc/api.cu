@@ -667,6 +667,68 @@ int scrub(Context* c, const uint32_t* data, size_t dpitch, size_t N, const uint3
     return 0;
 }
 
+// The scrub of a stripe with the f = |E| >= 1 blocks of the pattern R known lost (DESIGN 3j), on scrub()'s workspace and with its
+// two syncs: the fold of the surviving rows only, reduce, encode, u = s * cs (zero on the lost parity rows), inverse order-M
+// transform and the check of [f, M) (flag 0: not clean); Berlekamp-Massey on U^_f .. U^_(f + 2 max_bad - 1) of fold 0; C's order-M
+// transform, its roots at the surviving parity points, the product with u, the inverse transform and the check of [f + L, M); the
+// order-N transform of C_k rho^-k and its roots at the surviving data points.  The outputs are written as scrub() writes them.
+int scrub_degraded(Context* c, const fastecc_b200_repair* R, const uint32_t* data, size_t dpitch, const uint32_t* parity, size_t ppitch, size_t size,
+                   size_t max_bad, uint64_t seed, cudaStream_t st, int* status, uint32_t* bad_data, size_t* n_bad_data, uint32_t* bad_parity,
+                   size_t* n_bad_parity)
+{
+    const size_t N = R->N, M = R->M, f = R->ned + R->nep, rows = N + M, cap = max_bad ? max_bad : 1;
+    Lease ws(&c->repair, st);
+    CUDA_TRY(ws.acquire((rows * 4 + 4 + 2 * cap) * sizeof(uint32_t)));
+    uint32_t *x = ws.ptr(), *flags = x + rows * 4, *list_d = flags + 4, *list_p = list_d + cap;
+    CUDA_TRY(cudaMemsetAsync(x, 0, (rows * 4 + 4) * sizeof(uint32_t), st));
+    CUDA_TRY(launch_degraded_fold(data, dpitch, N, parity, ppitch, M, size, seed, R->d_lost, R->d_cs, x, c->num_sms, st)); g_launches++;
+    CUDA_TRY(launch_scrub_reduce(x, rows, st)); g_launches++;
+    TRY_RC(encode(c, x, N, M, 2, 4, st));
+    CUDA_TRY(launch_degraded_syndrome(x, N, M, R->d_cs, st)); g_launches++;
+    TRY_RC(ntt(c, x, M, 2, 4, true, st));                                      // 1 <= f < M: M >= 2
+    CUDA_TRY(launch_scrub_check(x, f, M, flags, st)); g_launches++;
+    uint32_t h[4];
+    std::vector<uint32_t> S(2 * max_bad);
+    CUDA_TRY(cudaMemcpyAsync(h, flags, sizeof h, cudaMemcpyDeviceToHost, st));
+    if (max_bad) CUDA_TRY(cudaMemcpy2DAsync(S.data(), 4, x + f * 4, 16, 4, S.size(), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    auto result = [&](int s) { *status = s; *n_bad_data = *n_bad_parity = 0; return 0; };
+    if (!h[0]) return result(FASTECC_B200_SCRUB_CLEAN);
+    if (!max_bad) return result(FASTECC_B200_SCRUB_DETECTED);
+    std::vector<uint32_t> C;
+    const size_t L = berlekamp_massey(S, C);
+    if (L > max_bad || C.size() != L + 1) return result(FASTECC_B200_SCRUB_DETECTED);
+    // the parity points zeta^j: C(zeta^j), then INTT_M(C(zeta^j) * u_j) in both folds
+    CUDA_TRY(cudaMemsetAsync(x, 0, M * 16, st));
+    CUDA_TRY(cudaMemcpy2DAsync(x, 16, C.data(), 4, 4, L + 1, cudaMemcpyHostToDevice, st));
+    TRY_RC(ntt(c, x, M, 2, 4, false, st));
+    CUDA_TRY(launch_degraded_roots(x, M, nullptr, R->d_cs, list_p, flags + 3, cap, st)); g_launches++;
+    CUDA_TRY(launch_scrub_product(x, N, M, st)); g_launches++;
+    TRY_RC(ntt(c, x, M, 2, 4, true, st));
+    CUDA_TRY(launch_scrub_check(x, f + L, M, flags + 1, st)); g_launches++;
+    // the data points omega^i: C(rho^-1 omega^i) = NTT_N(C_k rho^-k)[i]
+    const uint32_t rho_inv = gf::inv(gf::root((uint32_t)(2 * N)));
+    std::vector<uint32_t> T(L + 1);
+    for (size_t k = 0, r = 1; k <= L; ++k, r = gf::mulmod((uint32_t)r, rho_inv)) T[k] = gf::mulmod(C[k], (uint32_t)r);
+    CUDA_TRY(cudaMemsetAsync(x, 0, N * 16, st));
+    CUDA_TRY(cudaMemcpy2DAsync(x, 16, T.data(), 4, 4, L + 1, cudaMemcpyHostToDevice, st));
+    TRY_RC(ntt(c, x, N, 2, 4, false, st));                                     // N >= M >= 2
+    CUDA_TRY(launch_degraded_roots(x, N, R->d_lost, nullptr, list_d, flags + 2, cap, st)); g_launches++;
+    std::vector<uint32_t> ld(cap), lp(cap);
+    CUDA_TRY(cudaMemcpyAsync(h, flags, sizeof h, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(ld.data(), list_d, cap * 4, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(lp.data(), list_p, cap * 4, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    if (h[1] || (size_t)h[2] + h[3] != L) return result(FASTECC_B200_SCRUB_DETECTED);   // C fails the check, or a root is no surviving point
+    std::sort(ld.begin(), ld.begin() + h[2]);
+    std::sort(lp.begin(), lp.begin() + h[3]);
+    std::copy(ld.begin(), ld.begin() + h[2], bad_data);
+    std::copy(lp.begin(), lp.begin() + h[3], bad_parity);
+    *n_bad_data = h[2]; *n_bad_parity = h[3];
+    *status = FASTECC_B200_SCRUB_LOCATED;
+    return 0;
+}
+
 } // namespace
 
 namespace fecc {
@@ -963,6 +1025,30 @@ int fastecc_b200_rs_scrub(const uint32_t* d_data, size_t data_pitch, size_t N, c
     if (max_bad && (!bad_data || !bad_parity)) return fail(FASTECC_B200_EINVAL, "%s: null list of bad blocks", who);
     return scrub(c, d_data, data_pitch, N, d_parity, parity_pitch, M, size, max_bad, seed, (cudaStream_t)stream, status, bad_data, n_bad_data, bad_parity,
                  n_bad_parity);
+}
+
+int fastecc_b200_rs_scrub_degraded(const fastecc_b200_repair* R, const uint32_t* d_data, size_t data_pitch, const uint32_t* d_parity, size_t parity_pitch,
+                                   size_t size, size_t max_bad, uint64_t seed, void* stream, int* status, uint32_t* bad_data, size_t* n_bad_data,
+                                   uint32_t* bad_parity, size_t* n_bad_parity)
+{
+    const char* who = "fastecc_b200_rs_scrub_degraded";
+    Context* c = ctx(who);
+    if (!c) return FASTECC_B200_ENOINIT;
+    if (!R) return fail(FASTECC_B200_EINVAL, "%s: null pattern", who);
+    if (!status || !n_bad_data || !n_bad_parity) return fail(FASTECC_B200_EINVAL, "%s: null status or count output", who);
+    const size_t N = R->N, M = R->M, f = R->ned + R->nep;
+    if (f == M) return fail(FASTECC_B200_EINVAL, "%s: the pattern loses f = M = %zu blocks; no check symbol is left", who, M);
+    if (int rc = check_order(N, M, size, padded_pitch(size), FASTECC_B200_MAX_LOG_N_ENCODE, true, who)) return rc;
+    if (int rc = check_rows(d_data, N, size, data_pitch, true, who)) return rc;
+    if (int rc = check_rows(d_parity, M, size, parity_pitch, true, who)) return rc;
+    const size_t top = (M - f) / 2 < kMaxScrubBad ? (M - f) / 2 : kMaxScrubBad;
+    if (max_bad > top) return fail(FASTECC_B200_EINVAL, "%s: max_bad=%zu must be at most min((M - f) / 2, %zu) = %zu (M=%zu, f=%zu lost)", who, max_bad, kMaxScrubBad, top, M, f);
+    if (max_bad && (!bad_data || !bad_parity)) return fail(FASTECC_B200_EINVAL, "%s: null list of bad blocks", who);
+    if (!f)
+        return scrub(c, d_data, data_pitch, N, d_parity, parity_pitch, M, size, max_bad, seed, (cudaStream_t)stream, status, bad_data, n_bad_data, bad_parity,
+                     n_bad_parity);
+    return scrub_degraded(c, R, d_data, data_pitch, d_parity, parity_pitch, size, max_bad, seed, (cudaStream_t)stream, status, bad_data, n_bad_data,
+                          bad_parity, n_bad_parity);
 }
 
 int fastecc_b200_pin_host_buffers(int enable)

@@ -8,6 +8,9 @@
 // fold 0 gives C = L / L_0, which is trusted only if M * (C * S^ mod z^M - 1) vanishes on [deg C, M) in both folds and C has
 // deg C distinct roots among zeta^j (parity) and rho^-1 omega^i (data).  This file holds the fold, the element-wise kernels on
 // the single-column workspace and Berlekamp-Massey; api.cu runs them around the encode and the transforms.
+// The degraded scrub (fastecc_b200_rs_scrub_degraded, DESIGN 3j) is the same with f known lost blocks: their rows are never
+// loaded, the syndrome is weighted by the erasure locator (u_j = s_j * cs_j, zero on the lost parity rows), the checks start at f
+// and f + L, and the root search skips the lost points.
 #include "scrub.h"
 #include "gf.cuh"
 
@@ -46,9 +49,11 @@ constexpr uint32_t kFoldUnroll = 4;
 #define FOLD_MUL(b, t) gf::mul(b, (t)[0], (t)[1], (t)[2], zero)
 #endif
 
-__global__ void __launch_bounds__(256, 4) scrub_fold_kernel(const uint32_t* __restrict__ data, size_t dpitch, uint32_t N, const uint32_t* __restrict__ parity,
-                                                            size_t ppitch, uint32_t rows, uint32_t size, uint32_t s4, uint32_t log_w, uint32_t tiles,
-                                                            uint32_t items, uint32_t slice_rows, uint64_t seed, unsigned long long* __restrict__ ws)
+// The fold's body, shared by the plain and the degraded scrub: a row m with skip(m) is never loaded and folds to 0.
+template <class Skip>
+__device__ __forceinline__ void fold_rows(const uint32_t* __restrict__ data, size_t dpitch, uint32_t N, const uint32_t* __restrict__ parity, size_t ppitch,
+                                          uint32_t rows, uint32_t size, uint32_t s4, uint32_t log_w, uint32_t tiles, uint32_t items, uint32_t slice_rows,
+                                          uint64_t seed, unsigned long long* __restrict__ ws, Skip skip)
 {
     const uint32_t lane = threadIdx.x % 32, W = 1u << log_w, sub = lane & (W - 1), rw = 32 >> log_w, rlane = lane >> log_w;
     const uint32_t nwarps = gridDim.x * (blockDim.x / 32);
@@ -75,7 +80,7 @@ __global__ void __launch_bounds__(256, 4) scrub_fold_kernel(const uint32_t* __re
             for (uint32_t u = 0; u < kFoldUnroll; ++u) {
                 const uint32_t m = base + u * rw + rlane;
                 v[u] = make_uint4(0, 0, 0, 0);
-                if (live && m < r1) {
+                if (live && m < r1 && !skip(m)) {
                     const uint32_t* row = m < N ? data + (size_t)m * dpitch : parity + (size_t)(m - N) * ppitch;
                     v[u] = __ldg(reinterpret_cast<const uint4*>(row) + c);
                 }
@@ -105,6 +110,23 @@ __global__ void __launch_bounds__(256, 4) scrub_fold_kernel(const uint32_t* __re
     }
 }
 
+__global__ void __launch_bounds__(256, 4) scrub_fold_kernel(const uint32_t* __restrict__ data, size_t dpitch, uint32_t N, const uint32_t* __restrict__ parity,
+                                                            size_t ppitch, uint32_t rows, uint32_t size, uint32_t s4, uint32_t log_w, uint32_t tiles,
+                                                            uint32_t items, uint32_t slice_rows, uint64_t seed, unsigned long long* __restrict__ ws)
+{
+    fold_rows(data, dpitch, N, parity, ppitch, rows, size, s4, log_w, tiles, items, slice_rows, seed, ws, [](uint32_t) { return false; });
+}
+
+// The fold of a degraded stripe: the lost data rows (lost[m] != 0) and the lost parity rows (cs[j].x == 0) are never loaded.
+__global__ void __launch_bounds__(256, 4) degraded_fold_kernel(const uint32_t* __restrict__ data, size_t dpitch, uint32_t N, const uint32_t* __restrict__ parity,
+                                                               size_t ppitch, uint32_t rows, uint32_t size, uint32_t s4, uint32_t log_w, uint32_t tiles,
+                                                               uint32_t items, uint32_t slice_rows, uint64_t seed, unsigned long long* __restrict__ ws,
+                                                               const uint8_t* __restrict__ lost, const uint4* __restrict__ cs)
+{
+    fold_rows(data, dpitch, N, parity, ppitch, rows, size, s4, log_w, tiles, items, slice_rows, seed, ws,
+              [=](uint32_t m) { return m < N ? __ldg(lost + m) != 0 : __ldg(&cs[m - N].x) == 0u; });
+}
+
 __global__ void scrub_reduce_kernel(uint4* __restrict__ ws, size_t n)
 {
     FOR_GRID(size_t, i, n) {
@@ -121,6 +143,29 @@ __global__ void scrub_syndrome_kernel(uint4* __restrict__ ws, size_t N, size_t M
         ws[N + j] = s;
         ws[j] = s;
         if (s.x | s.y) *nonzero = 1;
+    }
+}
+
+// u_j = (ws[N + j] - ws[j]) * cs_j in both folds, into rows N + j and j; cs_j = 0 on a lost parity row, so u_j = 0 there
+__global__ void degraded_syndrome_kernel(uint4* __restrict__ ws, size_t N, size_t M, const uint4* __restrict__ cs)
+{
+    const uint32_t zero = gf::opaque_zero();
+    FOR_GRID(size_t, j, M) {
+        const uint4 p = ws[N + j], g = ws[j], k = __ldg(cs + j);
+        const uint4 u = make_uint4(gf::mulc(gf::sub(p.x, g.x), k, zero), gf::mulc(gf::sub(p.y, g.y), k, zero), 0u, 0u);
+        ws[N + j] = u;
+        ws[j] = u;
+    }
+}
+
+// scrub_roots_kernel over the surviving points only: row i is skipped if lost[i] != 0 or cs[i].x == 0 (either may be null)
+__global__ void degraded_roots_kernel(const uint4* __restrict__ ws, size_t n, const uint8_t* __restrict__ lost, const uint4* __restrict__ cs,
+                                      uint32_t* __restrict__ list, uint32_t* __restrict__ count, size_t cap)
+{
+    FOR_GRID(size_t, i, n) {
+        if (ws[i].x || (lost && lost[i]) || (cs && !cs[i].x)) continue;
+        const uint32_t k = atomicAdd(count, 1u);
+        if (k < cap) list[k] = (uint32_t)i;
     }
 }
 
@@ -158,6 +203,12 @@ namespace fecc {
 cudaError_t launch_scrub_fold(const uint32_t* data, size_t dpitch, size_t N, const uint32_t* parity, size_t ppitch, size_t M, size_t size,
                               uint64_t seed, uint32_t* ws, int num_sms, cudaStream_t st)
 {
+    return launch_degraded_fold(data, dpitch, N, parity, ppitch, M, size, seed, nullptr, nullptr, ws, num_sms, st);
+}
+
+cudaError_t launch_degraded_fold(const uint32_t* data, size_t dpitch, size_t N, const uint32_t* parity, size_t ppitch, size_t M, size_t size,
+                                 uint64_t seed, const uint8_t* lost, const uint4* cs, uint32_t* ws, int num_sms, cudaStream_t st)
+{
     const uint32_t s4 = (uint32_t)((size + 3) / 4), rows = (uint32_t)(N + M);
     uint32_t log_w = 0;
     while (log_w < 5 && (1u << log_w) < s4) ++log_w;
@@ -169,8 +220,26 @@ cudaError_t launch_scrub_fold(const uint32_t* data, size_t dpitch, size_t N, con
     const uint32_t slice_rows = (uint32_t)((groups + slices - 1) / slices * rw);
     slices = (rows + slice_rows - 1) / slice_rows;
     const size_t items = tiles * slices, blocks = (items + 7) / 8 < max_blocks ? (items + 7) / 8 : max_blocks;
-    scrub_fold_kernel<<<(unsigned)blocks, 256, 0, st>>>(data, dpitch, (uint32_t)N, parity, ppitch, rows, (uint32_t)size, s4, log_w, tiles,
-                                                        (uint32_t)items, slice_rows, seed, reinterpret_cast<unsigned long long*>(ws));
+    unsigned long long* const sums = reinterpret_cast<unsigned long long*>(ws);
+    if (lost)
+        degraded_fold_kernel<<<(unsigned)blocks, 256, 0, st>>>(data, dpitch, (uint32_t)N, parity, ppitch, rows, (uint32_t)size, s4, log_w, tiles,
+                                                               (uint32_t)items, slice_rows, seed, sums, lost, cs);
+    else
+        scrub_fold_kernel<<<(unsigned)blocks, 256, 0, st>>>(data, dpitch, (uint32_t)N, parity, ppitch, rows, (uint32_t)size, s4, log_w, tiles,
+                                                            (uint32_t)items, slice_rows, seed, sums);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_degraded_syndrome(uint32_t* ws, size_t N, size_t M, const uint4* cs, cudaStream_t st)
+{
+    degraded_syndrome_kernel<<<grid_size(M, 4096), 256, 0, st>>>(reinterpret_cast<uint4*>(ws), N, M, cs);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_degraded_roots(const uint32_t* ws, size_t n, const uint8_t* lost, const uint4* cs, uint32_t* list, uint32_t* count, size_t cap,
+                                  cudaStream_t st)
+{
+    degraded_roots_kernel<<<grid_size(n, 4096), 256, 0, st>>>(reinterpret_cast<const uint4*>(ws), n, lost, cs, list, count, cap);
     return cudaGetLastError();
 }
 

@@ -262,8 +262,7 @@ class Repair(_CPattern):
         self._h, self.N, self.M = h, int(N), int(M)
         self.lost_data, self.lost_parity = d.tolist(), p.tolist()
 
-    def repair(self, data, parity):
-        """data: [N, S] and parity: [M, S] int32 CUDA tensors (unit word stride), repaired in place."""
+    def _stripe(self, data, parity):
         if self._h is None:
             raise ValueError("the pattern was closed")
         (dp, dn, S, dpitch, stream), (pp, pn, ps, ppitch, _) = self._fe._dev_args(data), self._fe._dev_args(parity)
@@ -272,7 +271,27 @@ class Repair(_CPattern):
                 raise ValueError("%s has %d rows, the pattern was built for %d" % (name, rows, want))
         if S != ps:
             raise ValueError("data and parity rows differ in length: %d and %d words" % (S, ps))
+        return dp, dpitch, pp, ppitch, S, stream
+
+    def repair(self, data, parity):
+        """data: [N, S] and parity: [M, S] int32 CUDA tensors (unit word stride), repaired in place."""
+        dp, dpitch, pp, ppitch, S, stream = self._stripe(data, parity)
         self._fe._check(self._lib.fastecc_b200_rs_repair(self._h, dp, dpitch, pp, ppitch, S, stream))
+
+    def scrub(self, data, parity, max_bad: int = 0, seed: int = 0):
+        """Check the surviving blocks of the stripe before repair() trusts them (fastecc_b200_rs_scrub_degraded, DESIGN 3j): the
+        lost rows are never read.  Returns (status, bad_data, bad_parity) as rs_scrub_dev does, the lists naming corrupted survivors
+        only (max_bad at most min((M - f) // 2, 4096), f = the lost blocks).  LOCATED: repair with Repair(N, M, lost + located);
+        CLEAN: repair with this pattern.  Synchronises the current stream."""
+        import ctypes
+        import numpy as np
+        dp, dpitch, pp, ppitch, S, stream = self._stripe(data, parity)
+        cap = max(int(max_bad), 1)
+        bd, bp = np.zeros(cap, dtype=np.uint32), np.zeros(cap, dtype=np.uint32)
+        status, nd, npar = ctypes.c_int(-1), ctypes.c_size_t(0), ctypes.c_size_t(0)
+        self._fe._check(self._lib.fastecc_b200_rs_scrub_degraded(self._h, dp, dpitch, pp, ppitch, S, int(max_bad), int(seed) & ((1 << 64) - 1), stream,
+                                                                 ctypes.byref(status), bd.ctypes.data, ctypes.byref(nd), bp.ctypes.data, ctypes.byref(npar)))
+        return status.value, [int(x) for x in bd[:nd.value]], [int(x) for x in bp[:npar.value]]
 
 
 def decode(code, erased, be=None):

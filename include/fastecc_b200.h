@@ -236,6 +236,29 @@ int fastecc_b200_rs_scrub(const uint32_t* d_data, size_t data_pitch_words, size_
                           size_t SIZE_words, size_t max_bad, uint64_t seed, void* stream, int* status,
                           uint32_t* bad_data, size_t* n_bad_data, uint32_t* bad_parity, size_t* n_bad_parity);
 
+/* ---- scrub of a degraded stripe: some blocks known lost, the survivors checked ---------------------------------------
+ * The stripe of fastecc_b200_rs_scrub with the f = n_lost_data + n_lost_parity blocks of `known` (a pattern of
+ * fastecc_b200_rs_repair_pattern, which gives N and M) lost, 1 <= f < M.  Errors-and-erasures decoding (DESIGN 3j): a known lost
+ * block costs one check symbol, a corrupted survivor two, so the survivors alone detect up to M - f corrupted blocks and locate up
+ * to floor((M - f) / 2) of them, where fastecc_b200_rs_scrub, blind to the losses, reads the lost rows as corruption.  Use it
+ * before a repair: a repair from a corrupted survivor rebuilds wrong blocks and reports nothing.
+ *   Buffers, SIZE_words, seed (the fold weights), statuses and outputs as fastecc_b200_rs_scrub; nothing is written into the
+ *   buffers, which may overlap.  The rows of the lost blocks are never read: they may hold anything.
+ *   max_bad:  0 = detect only; else at most min(floor((M - f) / 2), FASTECC_B200_SCRUB_MAX_BAD).
+ *   Out:      the lists name surviving blocks only, ascending.  LOCATED: repair with a pattern of lost + located blocks (at most
+ *             f + max_bad <= M); CLEAN: repair with `known` itself.
+ * Guarantees, with t corrupted surviving blocks, each up to a probability of P^-2 over the folds' weights:
+ *   t = 0 -> CLEAN;  1 <= t <= max_bad -> LOCATED with exactly the corrupted survivors;  max_bad < t <= M - f - max_bad ->
+ *   DETECTED;  1 <= t <= M - f -> never CLEAN.  (Two error patterns off the lost blocks differ by a code word of the code
+ *   punctured on them, of distance M + 1 - f.)
+ * EINVAL, before anything is allocated or launched: a null pattern, status or count; f = M (nothing left to check); max_bad
+ * above its bound; null lists with max_bad > 0; the rows and pitches fastecc_b200_rs_scrub rejects.  A pattern with nothing lost
+ * runs fastecc_b200_rs_scrub itself.  Synchronises the stream; device memory as fastecc_b200_rs_scrub. */
+int fastecc_b200_rs_scrub_degraded(const fastecc_b200_repair* known, const uint32_t* d_data, size_t data_pitch_words,
+                                   const uint32_t* d_parity, size_t parity_pitch_words, size_t SIZE_words, size_t max_bad, uint64_t seed,
+                                   void* stream, int* status, uint32_t* bad_data, size_t* n_bad_data, uint32_t* bad_parity,
+                                   size_t* n_bad_parity);
+
 /* ---- one transform sharded over several GPUs (one process per GPU; BASELINE config 4) ---------------------------
  * Global block i = l*n_ranks + rank is local block l (data in, parity out).  An encode is: pass 0 on every rank,
  * all-to-all of whole blocks, pass 1, all-to-all, pass 2 -- the exchange is the caller's (fastecc_b200/sharded.py does it

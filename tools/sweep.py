@@ -4,7 +4,8 @@ encode at N = 2^7 .. 2^19 and forward NTT at N = 2^10 .. 2^20, 4096-byte blocks,
 calls.  Arrays below ~100 MB stay in the 126 MB L2 between calls (marked); the small orders are launch-latency bound.
 Then recoding, decoding, the asymmetric encode, the encode of 3 * 2^k / 9 * 2^k blocks (`encode_mixed`, DESIGN 3e) and
 their encode into fewer parity blocks (`encode_asym_mixed`, DESIGN 3f; `--asym-mixed`: only these).  `--repair`: only the repair
-of a stored stripe against the 2N-row decoder (DESIGN 3g); `--update`, `--scrub`: only the update (3h) or the scrub (3i) lines.
+of a stored stripe against the 2N-row decoder (DESIGN 3g); `--update`, `--scrub`, `--scrub-degraded`: only the update (3h), the
+scrub (3i) or the degraded scrub (3j) lines.
 Prints one JSON line per point."""
 import json
 import os
@@ -426,7 +427,75 @@ def scrub_sweep():
     shutil.rmtree(tmp, ignore_errors=True)
 
 
+def scrub_degraded_sweep():
+    """Scrub of a degraded stripe (fastecc_b200_rs_scrub_degraded through decoder.Repair.scrub, DESIGN 3j) against the plain
+    rs_scrub_dev of the same stripe with its lost rows intact, the two alternated twice in one session (the lower figures).  The
+    whole call: CUDA events around `reps` back-to-back calls (each synchronises the stream itself).  The fold alone: the device
+    time of degraded_fold_kernel / scrub_fold_kernel in a torch.profiler trace of the same calls.  f lost blocks (half data, half
+    parity), t corrupted survivors (half data, half parity), max_bad = min((M - f) / 2, 4096) for the degraded scrub and
+    min(M / 2, 4096) for the plain one; the fold's expected share of the plain fold's bytes is (N + M - f) / (N + M).  Each line
+    names the card and its power limit, read in the same run."""
+    from torch.profiler import ProfilerActivity, profile
+    from bench import gpu_identity
+    from fastecc_b200.decoder import Repair
+    fe.init(0)
+    card = gpu_identity(torch.cuda.current_device())
+
+    def fold_ms(fn, kernel, reps):
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(reps):
+                fn()
+            torch.cuda.synchronize()
+        us = [e.device_time_total for e in prof.key_averages() if kernel in e.key]
+        return us[0] / 1000 / reps if us else float("nan")
+
+    S, reps = 1024, 5
+    rng = np.random.default_rng(2)
+    for N, M in ((1 << 19, 1 << 19), (1 << 19, 1 << 15), (3 << 19, 1 << 19)):
+        data = (torch.arange(N * S, device="cuda", dtype=torch.int64) * 2654435761 % P).to(torch.int32).view(N, S)
+        buf = data.clone()
+        fe.rs_encode_asym_mixed_dev(buf, M)
+        parity = buf[:M].clone()
+        del buf
+        torch.cuda.empty_cache()
+        for f in (1, 16, M // 4):
+            fd = f // 2
+            lost_d = np.sort(rng.choice(N, size=fd, replace=False)); lost_p = np.sort(rng.choice(M, size=f - fd, replace=False))
+            rep = Repair(N, M, lost_d, lost_p)
+            max_bad, plain_bad = min((M - f) // 2, 4096), min(M // 2, 4096)
+            sd, sp = np.setdiff1d(np.arange(N), lost_d), np.setdiff1d(np.arange(M), lost_p)
+            for t in (0, 1, 16):
+                nd = t // 2
+                bd = np.sort(rng.choice(sd, size=nd, replace=False)); bp = np.sort(rng.choice(sp, size=t - nd, replace=False))
+                keep_d, keep_p = data[bd].clone(), parity[bp].clone()
+                data[bd] ^= 1; parity[bp] ^= 2
+                calls = {"degraded": (lambda: rep.scrub(data, parity, max_bad, 7), "degraded_fold_kernel"),
+                         "plain": (lambda: fe.rs_scrub_dev(data, parity, plain_bad, 7), "scrub_fold_kernel")}
+                status = {name: fn()[0] for name, (fn, _) in calls.items()}
+                ms = {name: [] for name in calls}
+                fold = {name: [] for name in calls}
+                for _ in range(2):
+                    for name, (fn, kernel) in calls.items():
+                        ms[name].append(timed(fn, reps))
+                        fold[name].append(fold_ms(fn, kernel, reps))
+                line = {"op": "scrub_degraded", "N": N, "M": M, "f": f, "t": t, "max_bad": max_bad, "block_bytes": 4 * S,
+                        "status": status["degraded"], "status_plain": status["plain"], "expected_fold_share": round((N + M - f) / (N + M), 4),
+                        "gpu": card["name"], "power_limit_w": card["power_limit_w"]}
+                for name in calls:
+                    line.update({"scrub_ms_" + name: round(min(ms[name]), 4), "fold_ms_" + name: round(min(fold[name]), 4)})
+                line["call_ratio"] = round(line["scrub_ms_degraded"] / line["scrub_ms_plain"], 3)
+                line["fold_ratio"] = round(line["fold_ms_degraded"] / line["fold_ms_plain"], 3)
+                print(json.dumps(line), flush=True)
+                data[bd] = keep_d; parity[bp] = keep_p
+            rep.close()
+        del data, parity
+        torch.cuda.empty_cache()
+
+
 if __name__ == "__main__":
+    if "--scrub-degraded" in sys.argv:                        # only the degraded scrub lines
+        scrub_degraded_sweep()
+        sys.exit(0)
     if "--scrub" in sys.argv:                                 # only the scrub lines
         scrub_sweep()
         sys.exit(0)
