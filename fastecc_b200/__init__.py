@@ -73,6 +73,7 @@ def lib() -> ctypes.CDLL:
         L.fastecc_b200_rs_update.argtypes = [vp, sz, sz, vp, sz, sz, vp, sz, vp, sz, sz, vp]; L.fastecc_b200_rs_update.restype = ci
         L.fastecc_b200_rs_scrub.argtypes = [vp, sz, sz, vp, sz, sz, sz, sz, ctypes.c_uint64, vp, vp, vp, vp, vp, vp]; L.fastecc_b200_rs_scrub.restype = ci
         L.fastecc_b200_rs_scrub_degraded.argtypes = [vp, vp, sz, vp, sz, sz, sz, ctypes.c_uint64, vp, vp, vp, vp, vp, vp]; L.fastecc_b200_rs_scrub_degraded.restype = ci
+        L.fastecc_b200_rs_reconstruct.argtypes = [vp, sz, sz, vp, sz, sz, vp, sz, vp, sz, vp, sz, vp, sz, vp, sz, sz, vp]; L.fastecc_b200_rs_reconstruct.restype = ci
         L.fastecc_b200_rs_encode_shard_pass.argtypes = [vp, sz, ci, ci, sz, sz, ci, vp]; L.fastecc_b200_rs_encode_shard_pass.restype = ci
         L.fastecc_b200_rs_encode_shard_pass_p2p.argtypes = [vp, vp, sz, ci, ci, sz, sz, ci, vp]; L.fastecc_b200_rs_encode_shard_pass_p2p.restype = ci
         L.fastecc_b200_ntt_shard_pass_p2p.argtypes = [vp, vp, sz, ci, ci, sz, sz, ci, ci, vp]; L.fastecc_b200_ntt_shard_pass_p2p.restype = ci
@@ -325,6 +326,34 @@ def rs_scrub_degraded_dev(data, parity, lost_data, lost_parity, max_bad: int = 0
         return r.scrub(data, parity, max_bad, seed)
     finally:
         r.close()
+
+
+def rs_reconstruct_dev(data, parity, lost_data, lost_parity, want_data=None, want_parity=None, out=None):
+    """Degraded read of a stored stripe (fastecc_b200_rs_reconstruct, DESIGN 3k): data = the N data rows, parity = the M parity
+    rows of rs_encode_asym_mixed_dev (int32 CUDA tensors, 16-byte aligned rows with pitches that are multiples of 4 words), read
+    only; lost_data / lost_parity = the unavailable blocks (at most M in all); want_data / want_parity = the lost blocks to produce
+    (default: all of them; len(lost_data) + len(want_parity) <= 32).  Reads the surviving data rows and the len(lost_data) lowest
+    surviving parity rows only.  Row q of `out` receives want_data[q], then the wanted parity blocks; `out` defaults to a new
+    int32 tensor with rows of ceil4(SIZE) words.  Returns `out`.  Asynchronous on the current stream."""
+    import torch
+    from .decoder import _CPattern
+    (dp, N, S, dpitch, stream), (pp, M, ps, ppitch, _) = _dev_args(data), _dev_args(parity)
+    if S != ps:
+        raise ValueError("data and parity rows differ in length: %d and %d words" % (S, ps))
+    u32 = lambda v: _CPattern._u32(v, "block numbers in [0, 2^32)")
+    ld, lp = u32(lost_data), u32(lost_parity)
+    wd = ld if want_data is None else u32(want_data)
+    wp = lp if want_parity is None else u32(want_parity)
+    n = wd.size + wp.size
+    if out is None:
+        out = torch.empty((n, (S + 3) // 4 * 4), dtype=torch.int32, device=data.device)[:, :S]
+    optr, on, osz, opitch, _ = _dev_args(out)
+    if (on, osz) != (n, S):
+        raise ValueError("out is %d x %d words for %d wanted blocks of %d words" % (on, osz, n, S))
+    arr = lambda a: a.ctypes.data if a.size else None
+    _check(lib().fastecc_b200_rs_reconstruct(dp, dpitch, N, pp, ppitch, M, arr(ld), ld.size, arr(lp), lp.size, arr(wd), wd.size, arr(wp), wp.size,
+                                             optr, opitch, S, stream))
+    return out
 
 
 def bytes_to_gfp_dev(raw, words=None):

@@ -9,6 +9,7 @@
 #include "repair.h"
 #include "update.h"
 #include "scrub.h"
+#include "reconstruct.h"
 #include "locator.h"
 #include <cuda_runtime.h>
 #include <algorithm>
@@ -102,9 +103,9 @@ struct Context {
     SharedBuf scratch;   // Y buffer of the two-pass NTT and of the asymmetric encode
     SharedBuf packed;    // repacked copy for unaligned device layouts
     SharedBuf mixed;     // destination of the order-3 / order-9 step of the N = 3 * 2^k, 9 * 2^k transforms
-    SharedBuf repair;    // workspace of fastecc_b200_rs_repair: N + M rows of one column chunk; and of fastecc_b200_rs_update and _scrub
+    SharedBuf repair;    // workspace of fastecc_b200_rs_repair: N + M rows of one column chunk; and of fastecc_b200_rs_update, _scrub and _reconstruct
     struct HostList { uint32_t* p = nullptr; size_t cap = 0; cudaEvent_t copied = nullptr; };
-    std::vector<HostList> lists;         // page-locked copies of fastecc_b200_rs_update's changed lists (used under repair's lease)
+    std::vector<HostList> lists;         // page-locked copies of host arrays for rs_update and rs_reconstruct (used under repair's lease)
     size_t next_list = 0;                // the one to wait for next once there are kMaxLists
     DevBuf staging;      // device copy for the host (T**) entry points (serialised by g_host_mu)
     std::map<TableKey, std::vector<TableSlot>> tables;   // one slot per pass of the plan
@@ -512,31 +513,32 @@ int update_table(Context* c, size_t N, cudaStream_t st, const uint4** T)
     return 0;
 }
 
-// The caller's host list of k changed rows into d_idx without waiting for the stream: a pageable source could make
-// cudaMemcpyAsync synchronise, so the list goes through one of the context's page-locked buffers, one whose last copy has run.
-// While fewer than kMaxLists exist, a new one is added when none is free and large enough (one that is new because the list
+// The caller's host array of n words (update's changed rows, the lists and the combination of a reconstruct) into d_dst without
+// waiting for the stream: a pageable source could make cudaMemcpyAsync synchronise, so the array goes through one of the context's
+// page-locked buffers, one whose last copy has run.
+// While fewer than kMaxLists exist, a new one is added when none is free and large enough (one that is new because the array
 // outgrew them all is at least twice the largest); after that the buffers are taken in turn, waiting for the copy out of the
-// next one, so a caller that queues many updates behind long work holds at most kMaxLists of them.  Freeing page-locked memory
+// next one, so a caller that queues many calls behind long work holds at most kMaxLists of them.  Freeing page-locked memory
 // could synchronise the device, so a buffer is only replaced when it is too small.  The caller holds repair's lease.
 constexpr size_t kMaxLists = 8;
-int upload_list(Context* c, const uint32_t* changed, size_t k, uint32_t* d_idx, cudaStream_t st)
+int upload_list(Context* c, const uint32_t* src, size_t n, uint32_t* d_dst, cudaStream_t st)
 {
     Context::HostList* h = nullptr;
     size_t largest = 0;
     for (Context::HostList& b : c->lists) {
         largest = b.cap > largest ? b.cap : largest;
-        if (h || b.cap < k) continue;
+        if (h || b.cap < n) continue;
         const cudaError_t e = cudaEventQuery(b.copied);
         if (e == cudaSuccess) h = &b;
         else clear_cuda_error();                                     // cudaErrorNotReady: still in flight
     }
-    size_t cap = k <= largest ? k : k > 2 * largest ? k : 2 * largest;
+    size_t cap = n <= largest ? n : n > 2 * largest ? n : 2 * largest;
     if (cap < 4096) cap = 4096;
     if (!h && c->lists.size() >= kMaxLists) {
         h = &c->lists[c->next_list];
         c->next_list = (c->next_list + 1) % kMaxLists;
         CUDA_TRY(cudaEventSynchronize(h->copied));
-        if (h->cap < k) {
+        if (h->cap < n) {
             cudaFreeHost(h->p); h->p = nullptr; h->cap = 0;
             CUDA_TRY(cudaHostAlloc((void**)&h->p, cap * sizeof(uint32_t), cudaHostAllocDefault));
             h->cap = cap;
@@ -550,8 +552,8 @@ int upload_list(Context* c, const uint32_t* changed, size_t k, uint32_t* d_idx, 
         c->lists.push_back(b);
         h = &c->lists.back();
     }
-    memcpy(h->p, changed, k * sizeof(uint32_t));
-    CUDA_TRY(cudaMemcpyAsync(d_idx, h->p, k * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+    memcpy(h->p, src, n * sizeof(uint32_t));
+    CUDA_TRY(cudaMemcpyAsync(d_dst, h->p, n * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaEventRecord(h->copied, st));
     return 0;
 }
@@ -726,6 +728,98 @@ int scrub_degraded(Context* c, const fastecc_b200_repair* R, const uint32_t* dat
     std::copy(lp.begin(), lp.begin() + h[3], bad_parity);
     *n_bad_data = h[2]; *n_bad_parity = h[3];
     *status = FASTECC_B200_SCRUB_LOCATED;
+    return 0;
+}
+
+// The combination of a degraded read (DESIGN 3k), n_out x a Barrett triples, row q for output q.  pos = J (a parity blocks) then the
+// wanted parity blocks; E = the a lost data blocks.  T(j, e) = T[(D j - e) mod N] = -2 / (N (y_j z_e - 1)), y_j = rho^(2 D j + 1),
+// z_e = rho^-2e, rho = GF_Root(2N), equals update_table_kernel's canonical entry (one batch inversion for all of them).  A = T(J, E)
+// is a Cauchy matrix up to diagonal scalings (the points y_j and z_e^-1 are distinct), so Gauss-Jordan always finds a pivot.
+// Wanted data block E[k]: row k of A^-1.  Wanted parity block j: T(j, E) A^-1.
+std::vector<uint32_t> reconstruct_combination(size_t N, size_t D, const std::vector<uint32_t>& pos, const uint32_t* E, size_t a,
+                                              const uint32_t* want_d, size_t nwd, size_t nwp)
+{
+    using gf::mulmod;
+    const size_t nk = pos.size();
+    const uint32_t rho = gf::root((uint32_t)(2 * N)), n = (uint32_t)(N % gf::P);
+    std::vector<uint32_t> z(a), Tv(nk * a), pre(nk * a + 1, 1u);
+    for (size_t e = 0; e < a; ++e) z[e] = gf::powmod(rho, (2 * N - 2 * (uint64_t)E[e]) % (2 * N));
+    for (size_t k = 0; k < nk; ++k) {
+        const uint32_t y = gf::powmod(rho, 2 * D * (uint64_t)pos[k] + 1);
+        for (size_t e = 0; e < a; ++e) Tv[k * a + e] = mulmod(n, gf::sub(mulmod(y, z[e]), 1u));
+    }
+    for (size_t i = 0; i < nk * a; ++i) pre[i + 1] = mulmod(pre[i], Tv[i]);
+    uint32_t inv = gf::inv(pre[nk * a]);
+    for (size_t i = nk * a; i-- > 0;) {
+        const uint32_t t = mulmod(inv, pre[i]);
+        inv = mulmod(inv, Tv[i]);
+        Tv[i] = mulmod(gf::P - 2, t);
+    }
+    std::vector<uint32_t> A(Tv.begin(), Tv.begin() + a * a), X(a * a, 0u);  // [A | X], X from I to A^-1
+    for (size_t i = 0; i < a; ++i) X[i * a + i] = 1;
+    for (size_t col = 0; col < a; ++col) {
+        size_t p = col;
+        while (!A[p * a + col]) ++p;
+        for (size_t j = 0; j < a; ++j) { std::swap(A[p * a + j], A[col * a + j]); std::swap(X[p * a + j], X[col * a + j]); }
+        const uint32_t f = gf::inv(A[col * a + col]);
+        for (size_t j = 0; j < a; ++j) { A[col * a + j] = mulmod(A[col * a + j], f); X[col * a + j] = mulmod(X[col * a + j], f); }
+        for (size_t r = 0; r < a; ++r) {
+            const uint32_t m = A[r * a + col];
+            if (r == col || !m) continue;
+            for (size_t j = 0; j < a; ++j) {
+                A[r * a + j] = gf::sub(A[r * a + j], mulmod(m, A[col * a + j]));
+                X[r * a + j] = gf::sub(X[r * a + j], mulmod(m, X[col * a + j]));
+            }
+        }
+    }
+    std::vector<uint32_t> B((nwd + nwp) * a * 4);
+    auto put = [&](size_t q, size_t j, uint32_t w) { const gf::Tw t = gf::make_tw(w); uint32_t* b = &B[(q * a + j) * 4]; b[0] = t.w; b[1] = t.whi; b[2] = t.wlo; b[3] = 0; };
+    for (size_t q = 0, k = 0; q < nwd; ++q) {
+        while (E[k] != want_d[q]) ++k;
+        for (size_t j = 0; j < a; ++j) put(q, j, X[k * a + j]);
+    }
+    for (size_t m = 0; m < nwp; ++m)
+        for (size_t j = 0; j < a; ++j) {
+            uint64_t s = 0;
+            for (size_t k = 0; k < a; ++k) s += mulmod(Tv[(a + m) * a + k], X[k * a + j]);
+            put(nwd + m, j, (uint32_t)(s % gf::P));
+        }
+    return B;
+}
+
+// The degraded read of one stripe (DESIGN 3k) on the repair workspace: K = a + nwp rows of 64-bit sums of one column chunk, then
+// the uploaded words {B, pos, lost data}.  Per chunk: zero the sums, the pass over the surviving data rows, the combination.
+int reconstruct(Context* c, const uint32_t* data, size_t dpitch, size_t N, const uint32_t* parity, size_t ppitch, size_t M, const uint32_t* lost_d,
+                size_t a, const uint32_t* lost_p, size_t nlp, const uint32_t* want_d, size_t nwd, const uint32_t* want_p, size_t nwp, uint32_t* out,
+                size_t opitch, size_t size, cudaStream_t st)
+{
+    std::vector<uint32_t> pos;                                      // J: the a lowest surviving parity blocks, then the wanted ones
+    for (uint32_t j = 0, q = 0; pos.size() < a; ++j) {
+        while (q < nlp && lost_p[q] < j) ++q;
+        if (q == nlp || lost_p[q] != j) pos.push_back(j);
+    }
+    pos.insert(pos.end(), want_p, want_p + nwp);
+    const size_t nk = pos.size(), n_out = nwd + nwp, D = N / M;
+    std::vector<uint32_t> up = reconstruct_combination(N, D, pos, lost_d, a, want_d, nwd, nwp);
+    const size_t nb = up.size();
+    up.insert(up.end(), pos.begin(), pos.end());
+    up.insert(up.end(), lost_d, lost_d + a);
+    const size_t cap = kMaxRepairBytes / 8 / nk / 4 * 4, w = padded_pitch(size) <= cap ? padded_pitch(size) : cap;
+    const uint4* T = nullptr;
+    TRY_RC(update_table(c, N, st, &T));
+    Lease ws(&c->repair, st);
+    CUDA_TRY(ws.acquire(nk * w * 8 + up.size() * sizeof(uint32_t)));
+    unsigned long long* sums = (unsigned long long*)ws.ptr();
+    uint32_t* d_up = (uint32_t*)(sums + nk * w);
+    const uint4* B = (const uint4*)d_up;
+    const uint32_t *d_pos = d_up + nb, *d_lost = d_pos + nk;
+    TRY_RC(upload_list(c, up.data(), up.size(), d_up, st));
+    for (size_t c0 = 0; c0 < size; c0 += w) {
+        const size_t cols = size - c0 < w ? size - c0 : w;
+        CUDA_TRY(cudaMemsetAsync(sums, 0, nk * ((cols + 3) / 4 * 4) * 8, st));
+        CUDA_TRY(launch_reconstruct_sum(data + c0, dpitch, N, D, T, d_pos, nk, d_lost, a, cols, sums, c->num_sms, st)); g_launches++;
+        CUDA_TRY(launch_reconstruct_combine(sums, parity + c0, ppitch, d_pos, a, B, n_out, nwd, out + c0, opitch, cols, c->num_sms, st)); g_launches++;
+    }
     return 0;
 }
 
@@ -1049,6 +1143,40 @@ int fastecc_b200_rs_scrub_degraded(const fastecc_b200_repair* R, const uint32_t*
                      n_bad_parity);
     return scrub_degraded(c, R, d_data, data_pitch, d_parity, parity_pitch, size, max_bad, seed, (cudaStream_t)stream, status, bad_data, n_bad_data,
                           bad_parity, n_bad_parity);
+}
+
+int fastecc_b200_rs_reconstruct(const uint32_t* d_data, size_t data_pitch, size_t N, const uint32_t* d_parity, size_t parity_pitch, size_t M,
+                                const uint32_t* lost_data, size_t n_lost_data, const uint32_t* lost_parity, size_t n_lost_parity,
+                                const uint32_t* want_data, size_t n_want_data, const uint32_t* want_parity, size_t n_want_parity,
+                                uint32_t* d_out, size_t out_pitch, size_t size, void* stream)
+{
+    const char* who = "fastecc_b200_rs_reconstruct";
+    Context* c = ctx(who);
+    if (!c) return FASTECC_B200_ENOINIT;
+    if (int rc = check_order(N, M, size, padded_pitch(size), FASTECC_B200_MAX_LOG_N_ENCODE, true, who)) return rc;
+    if (int rc = check_rows(d_data, N, size, data_pitch, true, who)) return rc;
+    if (int rc = check_rows(d_parity, M, size, parity_pitch, true, who)) return rc;
+    if ((n_lost_data && !lost_data) || (n_lost_parity && !lost_parity) || (n_want_data && !want_data) || (n_want_parity && !want_parity))
+        return fail(FASTECC_B200_EINVAL, "%s: null block list", who);
+    if (!ascending_below(lost_data, n_lost_data, N) || !ascending_below(want_data, n_want_data, N))
+        return fail(FASTECC_B200_EINVAL, "%s: lost and wanted data blocks must be ascending, distinct and below N=%zu", who, N);
+    if (!ascending_below(lost_parity, n_lost_parity, M) || !ascending_below(want_parity, n_want_parity, M))
+        return fail(FASTECC_B200_EINVAL, "%s: lost and wanted parity blocks must be ascending, distinct and below M=%zu", who, M);
+    if (!std::includes(lost_data, lost_data + n_lost_data, want_data, want_data + n_want_data) ||
+        !std::includes(lost_parity, lost_parity + n_lost_parity, want_parity, want_parity + n_want_parity))
+        return fail(FASTECC_B200_EINVAL, "%s: every wanted block must be a lost one", who);
+    if (n_lost_data + n_lost_parity > M)
+        return fail(FASTECC_B200_EINVAL, "%s: %zu + %zu lost blocks exceed M=%zu", who, n_lost_data, n_lost_parity, M);
+    if (n_lost_data + n_want_parity > FASTECC_B200_RECONSTRUCT_MAX)
+        return fail(FASTECC_B200_EINVAL, "%s: n_lost_data + n_want_parity = %zu exceeds FASTECC_B200_RECONSTRUCT_MAX = %d; fastecc_b200_rs_repair rebuilds up "
+                    "to M lost blocks", who, n_lost_data + n_want_parity, FASTECC_B200_RECONSTRUCT_MAX);
+    const size_t n_out = n_want_data + n_want_parity;
+    if (!n_out) return 0;
+    if (int rc = check_rows(d_out, n_out, size, out_pitch, true, who)) return rc;
+    if (rows_overlap(d_out, n_out, out_pitch, d_data, N, data_pitch, size) || rows_overlap(d_out, n_out, out_pitch, d_parity, M, parity_pitch, size))
+        return fail(FASTECC_B200_EINVAL, "%s: the output overlaps the data or the parity buffer", who);
+    return reconstruct(c, d_data, data_pitch, N, d_parity, parity_pitch, M, lost_data, n_lost_data, lost_parity, n_lost_parity, want_data, n_want_data,
+                       want_parity, n_want_parity, d_out, out_pitch, size, (cudaStream_t)stream);
 }
 
 int fastecc_b200_pin_host_buffers(int enable)

@@ -148,6 +148,14 @@ GF_HD uint32_t opaque_zero()
 
 GF_HD uint32_t canon(uint32_t x) { return x >= P ? x - P : x; }
 
+// x mod P without a division: 2^32 = 2^20 - 1 mod P, so fold the high word down until none is left (the 64-bit sums of the
+// scrub's fold and of the degraded read).
+GF_HD uint32_t reduce64(uint64_t x)
+{
+    while (x >> 32) x = (x >> 32) * C + (x & 0xFFFFFFFFull);
+    return canon((uint32_t)x);
+}
+
 // a + b and a - b of canonical residues
 GF_HD uint32_t add(uint32_t a, uint32_t b) { const uint32_t s = a + b; return (s < a || s >= P) ? s - P : s; }
 GF_HD uint32_t sub(uint32_t a, uint32_t b) { return a >= b ? a - b : a + (P - b); }

@@ -19,20 +19,13 @@ namespace {
 using namespace fecc;
 constexpr uint32_t P = gf::P;
 
-// x mod P without a division: 2^32 = 2^20 - 1 mod P, so fold the high word down until none is left.
-__device__ __forceinline__ uint32_t reduce64(uint64_t x)
-{
-    while (x >> 32) x = (x >> 32) * gf::C + (x & 0xFFFFFFFFull);
-    return gf::canon((uint32_t)x);
-}
-
 // r_f,c: the (2c + f + 1)-th output of splitmix64 started at `seed`, mod P (include/fastecc_b200.h states it)
 __device__ __forceinline__ uint32_t fold_weight(uint64_t seed, uint32_t f, uint64_t c)
 {
     uint64_t z = seed + (2 * c + f + 1) * 0x9E3779B97F4A7C15ull;
     z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
     z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-    return reduce64(z ^ (z >> 31));
+    return gf::reduce64(z ^ (z >> 31));
 }
 
 // A work item is one tile of W 16-byte chunks (W = 32, or the next power of two >= ceil(SIZE / 4) for short rows) of every row
@@ -131,7 +124,7 @@ __global__ void scrub_reduce_kernel(uint4* __restrict__ ws, size_t n)
 {
     FOR_GRID(size_t, i, n) {
         const uint4 v = ws[i];
-        ws[i] = make_uint4(reduce64(((uint64_t)v.y << 32) | v.x), reduce64(((uint64_t)v.w << 32) | v.z), 0u, 0u);
+        ws[i] = make_uint4(gf::reduce64(((uint64_t)v.y << 32) | v.x), gf::reduce64(((uint64_t)v.w << 32) | v.z), 0u, 0u);
     }
 }
 

@@ -259,6 +259,34 @@ int fastecc_b200_rs_scrub_degraded(const fastecc_b200_repair* known, const uint3
                                    void* stream, int* status, uint32_t* bad_data, size_t* n_bad_data, uint32_t* bad_parity,
                                    size_t* n_bad_parity);
 
+/* ---- degraded read: a few lost blocks rebuilt out of place from N surviving rows ----------------------------------------
+ * The read of a stripe with blocks missing: the wanted lost blocks are computed into d_out, and nothing is written into the
+ * stripe.  The stripe is that of fastecc_b200_rs_repair (N data rows data_pitch_words apart, M parity rows parity_pitch_words
+ * apart, any (N, M) that fastecc_b200_rs_encode_asym_mixed_dev accepts).  It costs one pass over N rows and needs no pattern
+ * (DESIGN 3k).
+ *   Lists:    lost_data / lost_parity name the unavailable blocks; want_data / want_parity the blocks to produce, a subset of
+ *             them.  All are HOST arrays, ascending, distinct, below N or M.  With a = n_lost_data: a + n_lost_parity <= M, and
+ *             a + n_want_parity <= FASTECC_B200_RECONSTRUCT_MAX (fastecc_b200_rs_repair rebuilds more).
+ *   Rows read: exactly the N - a surviving data rows and the parity rows J = the a lowest-numbered parity blocks not in
+ *             lost_parity, so a storage layer fetches only those N blocks.  No other row is loaded: lost rows and parity rows
+ *             outside J may hold anything.  Words are taken mod P.
+ *   Out:      row q of d_out (out_pitch_words apart) receives block want_data[q] for q < n_want_data, then the blocks of
+ *             want_parity in order; words [0, SIZE) of those rows only, canonical.
+ * PRECONDITION: the surviving blocks are a consistent stripe (as for fastecc_b200_rs_update).  A corrupted survivor gives wrong
+ * blocks without a report; fastecc_b200_rs_scrub_degraded checks the survivors first.
+ * All three buffers 16-byte aligned with pitches that are multiples of 4 words; d_data and d_parity may overlap each other, d_out
+ * may overlap neither.  Validated in full before anything is allocated or launched (EINVAL).  Asynchronous on the stream, which it
+ * does not synchronise; the host lists may be freed as soon as the call returns.  n_want_data + n_want_parity == 0 returns 0 and
+ * launches nothing.  Two kernel launches per call (per column chunk), plus the build of fastecc_b200_rs_update's table at the first
+ * use of an N.  Device memory: that table (16 bytes per data block) and K * ceil4(SIZE) * 8 bytes of the context's repair
+ * workspace, K = a + n_want_parity; above 4 GiB the call runs in column chunks within that bound. */
+#define FASTECC_B200_RECONSTRUCT_MAX 32
+int fastecc_b200_rs_reconstruct(const uint32_t* d_data, size_t data_pitch_words, size_t N,
+                                const uint32_t* d_parity, size_t parity_pitch_words, size_t M,
+                                const uint32_t* lost_data, size_t n_lost_data, const uint32_t* lost_parity, size_t n_lost_parity,
+                                const uint32_t* want_data, size_t n_want_data, const uint32_t* want_parity, size_t n_want_parity,
+                                uint32_t* d_out, size_t out_pitch_words, size_t SIZE_words, void* stream);
+
 /* ---- one transform sharded over several GPUs (one process per GPU; BASELINE config 4) ---------------------------
  * Global block i = l*n_ranks + rank is local block l (data in, parity out).  An encode is: pass 0 on every rank,
  * all-to-all of whole blocks, pass 1, all-to-all, pass 2 -- the exchange is the caller's (fastecc_b200/sharded.py does it

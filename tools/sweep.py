@@ -4,8 +4,8 @@ encode at N = 2^7 .. 2^19 and forward NTT at N = 2^10 .. 2^20, 4096-byte blocks,
 calls.  Arrays below ~100 MB stay in the 126 MB L2 between calls (marked); the small orders are launch-latency bound.
 Then recoding, decoding, the asymmetric encode, the encode of 3 * 2^k / 9 * 2^k blocks (`encode_mixed`, DESIGN 3e) and
 their encode into fewer parity blocks (`encode_asym_mixed`, DESIGN 3f; `--asym-mixed`: only these).  `--repair`: only the repair
-of a stored stripe against the 2N-row decoder (DESIGN 3g); `--update`, `--scrub`, `--scrub-degraded`: only the update (3h), the
-scrub (3i) or the degraded scrub (3j) lines.
+of a stored stripe against the 2N-row decoder (DESIGN 3g); `--update`, `--scrub`, `--scrub-degraded`, `--reconstruct`: only the update (3h),
+the scrub (3i), the degraded scrub (3j) or the degraded read (3k) lines.
 Prints one JSON line per point."""
 import json
 import os
@@ -492,7 +492,71 @@ def scrub_degraded_sweep():
         torch.cuda.empty_cache()
 
 
+def reconstruct_sweep():
+    """Degraded read (fastecc_b200_rs_reconstruct, DESIGN 3k) against rs_repair_dev of the same stripe and losses (its pattern
+    built once, outside the timing), the two alternated twice in one session (the lower figures).  The call: CUDA events around
+    `reps` back-to-back calls.  The sum kernel: its device time in a torch.profiler trace of the same calls, and that time over
+    two floors: the memory floor (N * SIZE * 4 bytes at the data sheet's 3.35 TB/s) and the product floor (K * N * SIZE products at
+    the 1.7e12 products/s that update_parity_kernel measured, DESIGN 3h).  a lost data blocks, all wanted; "+p": one lost parity
+    block wanted as well (K = a + 1).  Each line names the card and its power limit, read in the same run."""
+    from torch.profiler import ProfilerActivity, profile
+    from bench import gpu_identity
+    from fastecc_b200.decoder import Repair
+    fe.init(0)
+    card = gpu_identity(torch.cuda.current_device())
+
+    def kernel_ms(fn, kernel, reps):
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(reps):
+                fn()
+            torch.cuda.synchronize()
+        us = [e.device_time_total for e in prof.key_averages() if kernel in e.key]
+        return sum(us) / 1000 / reps if us else float("nan")
+
+    S, reps = 1024, 5
+    rng = np.random.default_rng(3)
+    for N, M in ((1 << 19, 1 << 19), (1 << 19, 1 << 15), (3 << 19, 1 << 19), (9 << 18, 1 << 18)):
+        data = (torch.arange(N * S, device="cuda", dtype=torch.int64) * 2654435761 % P).to(torch.int32).view(N, S)
+        buf = data.clone()
+        fe.rs_encode_asym_mixed_dev(buf, M)
+        parity = buf[:M].clone()
+        del buf
+        torch.cuda.empty_cache()
+        for a in (1, 2, 4, 8, 16, 32):
+            for with_p in ((False, True) if a < 32 else (False,)):
+                lost_d = np.sort(rng.choice(N, size=a, replace=False))
+                lost_p = np.sort(rng.choice(M, size=1, replace=False)) if with_p else np.zeros(0, dtype=np.int64)
+                K = a + len(lost_p)
+                want = torch.cat([data[torch.as_tensor(lost_d, device="cuda")], parity[torch.as_tensor(lost_p, device="cuda")]])
+                out = fe.rs_reconstruct_dev(data, parity, lost_d, lost_p)
+                ok = bool(torch.equal(out, want))
+                rep = Repair(N, M, lost_d, lost_p)
+                calls = {"reconstruct": lambda: fe.rs_reconstruct_dev(data, parity, lost_d, lost_p, out=out),
+                         "repair": lambda: rep.repair(data, parity)}
+                ms = {name: [] for name in calls}
+                sum_ms = []
+                for _ in range(2):
+                    for name, fn in calls.items():
+                        ms[name].append(timed(fn, reps))
+                    sum_ms.append(kernel_ms(calls["reconstruct"], "reconstruct_sum_kernel", reps))
+                rep.close()
+                mem_floor = N * S * 4 / 3.35e12 * 1e3
+                prod_floor = K * N * S / 1.7e12 * 1e3
+                t = min(sum_ms)
+                print(json.dumps({"op": "reconstruct", "N": N, "M": M, "a": a, "want_parity": int(with_p), "K": K, "block_bytes": 4 * S, "ok": ok,
+                                  "call_ms": round(min(ms["reconstruct"]), 4), "sum_kernel_ms": round(t, 4),
+                                  "memory_floor_frac": round(mem_floor / t, 3), "product_floor_frac_at_update_rate": round(prod_floor / t, 3),
+                                  "repair_ms": round(min(ms["repair"]), 4), "speedup_vs_repair": round(min(ms["repair"]) / min(ms["reconstruct"]), 2),
+                                  "gpu": card["name"], "power_limit_w": card["power_limit_w"]}), flush=True)
+                del out, want
+        del data, parity
+        torch.cuda.empty_cache()
+
+
 if __name__ == "__main__":
+    if "--reconstruct" in sys.argv:                           # only the degraded read lines
+        reconstruct_sweep()
+        sys.exit(0)
     if "--scrub-degraded" in sys.argv:                        # only the degraded scrub lines
         scrub_degraded_sweep()
         sys.exit(0)
