@@ -74,6 +74,7 @@ def lib() -> ctypes.CDLL:
         L.fastecc_b200_rs_scrub.argtypes = [vp, sz, sz, vp, sz, sz, sz, sz, ctypes.c_uint64, vp, vp, vp, vp, vp, vp]; L.fastecc_b200_rs_scrub.restype = ci
         L.fastecc_b200_rs_scrub_degraded.argtypes = [vp, vp, sz, vp, sz, sz, sz, ctypes.c_uint64, vp, vp, vp, vp, vp, vp]; L.fastecc_b200_rs_scrub_degraded.restype = ci
         L.fastecc_b200_rs_reconstruct.argtypes = [vp, sz, sz, vp, sz, sz, vp, sz, vp, sz, vp, sz, vp, sz, vp, sz, sz, vp]; L.fastecc_b200_rs_reconstruct.restype = ci
+        L.fastecc_b200_rs_encode_batch.argtypes = [vp, sz, sz, sz, vp, sz, sz, sz, sz, sz, vp]; L.fastecc_b200_rs_encode_batch.restype = ci
         L.fastecc_b200_rs_encode_shard_pass.argtypes = [vp, sz, ci, ci, sz, sz, ci, vp]; L.fastecc_b200_rs_encode_shard_pass.restype = ci
         L.fastecc_b200_rs_encode_shard_pass_p2p.argtypes = [vp, vp, sz, ci, ci, sz, sz, ci, vp]; L.fastecc_b200_rs_encode_shard_pass_p2p.restype = ci
         L.fastecc_b200_ntt_shard_pass_p2p.argtypes = [vp, vp, sz, ci, ci, sz, sz, ci, ci, vp]; L.fastecc_b200_ntt_shard_pass_p2p.restype = ci
@@ -354,6 +355,31 @@ def rs_reconstruct_dev(data, parity, lost_data, lost_parity, want_data=None, wan
     _check(lib().fastecc_b200_rs_reconstruct(dp, dpitch, N, pp, ppitch, M, arr(ld), ld.size, arr(lp), lp.size, arr(wd), wd.size, arr(wp), wp.size,
                                              optr, opitch, S, stream))
     return out
+
+
+def rs_encode_batch_dev(data, parity=None, M=None):
+    """Encode a batch of small stripes in one launch (fastecc_b200_rs_encode_batch, DESIGN 3l): data = [B, N, S] CUDA int32/uint32
+    tensor with unit word stride (a view such as buf[:, :N, :S] of a [B, N + M, pitch] buffer is fine), read only; N <= 64 in the
+    family rs_encode_asym_mixed_dev accepts.  parity = [B, M, S] receives each stripe's M parity blocks, bit for bit those of
+    rs_encode_asym_mixed_dev on that stripe; when it is None, M must be given and a new int32 tensor with rows of ceil4(S) words is
+    allocated.  Rows 16-byte aligned with pitches and stripe strides that are multiples of 4 words; the parity may not overlap
+    itself or the data.  Returns `parity`.  Asynchronous on the current stream."""
+    import torch
+
+    def args(t, name):
+        if not (t.is_cuda and t.dim() == 3 and t.dtype in (torch.int32, torch.uint32) and t.stride(2) == 1):
+            raise ValueError("%s: expected a 3-D CUDA int32/uint32 tensor with unit stride along the word dimension" % name)
+        return t.data_ptr(), t.shape[0], t.shape[1], t.shape[2], t.stride(1), t.stride(0)
+    dp, B, N, S, dpitch, dstride = args(data, "data")
+    if parity is None:
+        if M is None:
+            raise ValueError("give the number of parity blocks M or a parity tensor")
+        parity = torch.empty((B, int(M), (S + 3) // 4 * 4), dtype=torch.int32, device=data.device)[..., :S]
+    pp, pB, pM, pS, ppitch, pstride = args(parity, "parity")
+    if (pB, pS) != (B, S) or (M is not None and pM != int(M)):
+        raise ValueError("parity is %d x %d x %d words for %d stripes of %s x %d-word blocks" % (pB, pM, pS, B, "M" if M is None else int(M), S))
+    _check(lib().fastecc_b200_rs_encode_batch(dp, dpitch, dstride, N, pp, ppitch, pstride, pM, B, S, torch.cuda.current_stream(data.device).cuda_stream))
+    return parity
 
 
 def bytes_to_gfp_dev(raw, words=None):

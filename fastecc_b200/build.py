@@ -6,7 +6,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libfastecc_b200.so")
-SOURCES = ["api.cu", "ntt_pass.cu", "small_dft.cu", "byte_recode.cu", "elementwise.cu", "decode.cu", "mixed_radix.cu", "repair.cu", "update.cu", "scrub.cu", "reconstruct.cu"]
+SOURCES = ["api.cu", "ntt_pass.cu", "small_dft.cu", "byte_recode.cu", "elementwise.cu", "decode.cu", "mixed_radix.cu", "repair.cu", "update.cu", "scrub.cu", "reconstruct.cu", "batch.cu"]
 HEADERS = sorted(f for f in os.listdir(CSRC) if f.endswith((".cuh", ".h"))) + [os.path.join("..", "..", "include", "fastecc_b200.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC,-O3", "-shared"]

@@ -10,6 +10,7 @@
 #include "update.h"
 #include "scrub.h"
 #include "reconstruct.h"
+#include "batch.h"
 #include "locator.h"
 #include <cuda_runtime.h>
 #include <algorithm>
@@ -1177,6 +1178,35 @@ int fastecc_b200_rs_reconstruct(const uint32_t* d_data, size_t data_pitch, size_
         return fail(FASTECC_B200_EINVAL, "%s: the output overlaps the data or the parity buffer", who);
     return reconstruct(c, d_data, data_pitch, N, d_parity, parity_pitch, M, lost_data, n_lost_data, lost_parity, n_lost_parity, want_data, n_want_data,
                        want_parity, n_want_parity, d_out, out_pitch, size, (cudaStream_t)stream);
+}
+
+int fastecc_b200_rs_encode_batch(const uint32_t* d_data, size_t data_pitch, size_t data_stride, size_t N, uint32_t* d_parity, size_t parity_pitch,
+                                 size_t parity_stride, size_t M, size_t n_stripes, size_t size, void* stream)
+{
+    const char* who = "fastecc_b200_rs_encode_batch";
+    Context* c = ctx(who);
+    if (!c) return FASTECC_B200_ENOINIT;
+    if (int rc = check_order(N, M, size, padded_pitch(size), FASTECC_B200_MAX_LOG_N_ENCODE, true, who)) return rc;
+    if (N > FASTECC_B200_BATCH_MAX_N)
+        return fail(FASTECC_B200_EINVAL, "%s: N=%zu exceeds FASTECC_B200_BATCH_MAX_N = %d; encode larger stripes one at a time with "
+                    "fastecc_b200_rs_encode_asym_mixed_dev", who, N, FASTECC_B200_BATCH_MAX_N);
+    if (data_pitch < size || parity_pitch < size)
+        return fail(FASTECC_B200_EINVAL, "%s: needs SIZE_words (%zu) <= data_pitch_words (%zu) and parity_pitch_words (%zu)", who, size, data_pitch, parity_pitch);
+    if ((uintptr_t)d_data % 16 || (uintptr_t)d_parity % 16 || data_pitch % 4 || parity_pitch % 4 || data_stride % 4 || parity_stride % 4)
+        return fail(FASTECC_B200_EINVAL, "%s: needs 16-byte aligned buffers and pitches and stripe strides that are multiples of 4 words", who);
+    if (!n_stripes) return 0;                                              // an empty batch reads and writes nothing: any pointers do
+    if (!d_data || !d_parity) return fail(FASTECC_B200_EINVAL, "%s: null device pointer", who);
+    if ((unsigned long long)n_stripes * ((size + 3) / 4) >= (1ull << 36))
+        return fail(FASTECC_B200_EINVAL, "%s: %zu stripes of %zu words exceed 2^36 16-byte chunks", who, n_stripes, size);
+    const BatchRows d{(uintptr_t)d_data / 4, data_pitch, data_stride, N}, p{(uintptr_t)d_parity / 4, parity_pitch, parity_stride, M};
+    if (!batch_layout_disjoint(d, p, n_stripes, size))
+        return fail(FASTECC_B200_EINVAL, "%s: parity rows may overlap each other or the data; accepted layouts: separate data and parity spans, each "
+                    "stripe-major or block-major, or one common stripe stride holding each stripe's N + M disjoint rows", who);
+    const cudaStream_t st = (cudaStream_t)stream;
+    const uint4* T = nullptr;
+    TRY_RC(update_table(c, N, st, &T));
+    CUDA_TRY(launch_batch_encode(d_data, data_pitch, data_stride, N, d_parity, parity_pitch, parity_stride, M, n_stripes, size, T, st)); g_launches++;
+    return 0;
 }
 
 int fastecc_b200_pin_host_buffers(int enable)

@@ -287,6 +287,31 @@ int fastecc_b200_rs_reconstruct(const uint32_t* d_data, size_t data_pitch_words,
                                 const uint32_t* want_data, size_t n_want_data, const uint32_t* want_parity, size_t n_want_parity,
                                 uint32_t* d_out, size_t out_pitch_words, size_t SIZE_words, void* stream);
 
+/* ---- encode of a batch of small stripes, out of place, in one launch ---------------------------------------------------
+ * The write of many stripes at once: for each of n_stripes stripes of N data blocks, its M parity blocks into rows of their own;
+ * the data is only read.  Data block i of stripe b is at d_data + b * data_stripe_words + i * data_pitch_words, parity block j of
+ * stripe b at d_parity + b * parity_stripe_words + j * parity_pitch_words.  N is any order that
+ * fastecc_b200_rs_encode_asym_mixed_dev accepts (2^k, 3 * 2^k or 9 * 2^k) up to FASTECC_B200_BATCH_MAX_N, M any divisor of N;
+ * larger stripes go through the per-stripe entry points.  Each parity block is M x N products per word straight from the data
+ * (fastecc_b200_rs_update's formula, DESIGN 3l), so the call pays one launch for the batch instead of a transform per stripe.
+ *   Result:  parity row j of every stripe equals row j of fastecc_b200_rs_encode_asym_mixed_dev run on that stripe's data, bit
+ *            for bit, so fastecc_b200_rs_repair, _update, _scrub and _reconstruct take the stripes as they are.
+ *   Writes:  words [0, SIZE) of the n_stripes * M parity rows, canonical, and nothing else: no data word, no pad word, no word
+ *            between rows.  Reads: the data, whose words are taken mod P; pad words past SIZE never enter a sum.
+ *   Layout:  both bases 16-byte aligned; the two pitches and the two stripe strides multiples of 4 words; each pitch >= SIZE.  No
+ *            parity word may be another parity word or a data word (data rows may overlap each other).  The call accepts only
+ *            layouts it proves disjoint in O(N + M) host work: separate data and parity spans with pairwise disjoint parity rows,
+ *            each side stripe-major ([B][N][pitch]) or block-major ([N][B][pitch]) in any combination; or one common stripe stride
+ *            in which stripe 0's N + M rows, in any order, are disjoint and fit inside one stride (e.g. [B][N + M][pitch] with the
+ *            parity below the data).  Anything else is EINVAL.
+ * Validated in full before anything is allocated or launched (EINVAL).  n_stripes == 0 returns 0 and launches nothing (null buffers included); otherwise
+ * one kernel launch, plus the build of fastecc_b200_rs_update's table at the first use of an N.  No workspace, no host-to-device
+ * copy.  Asynchronous on the stream, which it does not synchronise. */
+#define FASTECC_B200_BATCH_MAX_N 64
+int fastecc_b200_rs_encode_batch(const uint32_t* d_data, size_t data_pitch_words, size_t data_stripe_words, size_t N,
+                                 uint32_t* d_parity, size_t parity_pitch_words, size_t parity_stripe_words, size_t M,
+                                 size_t n_stripes, size_t SIZE_words, void* stream);
+
 /* ---- one transform sharded over several GPUs (one process per GPU; BASELINE config 4) ---------------------------
  * Global block i = l*n_ranks + rank is local block l (data in, parity out).  An encode is: pass 0 on every rank,
  * all-to-all of whole blocks, pass 1, all-to-all, pass 2 -- the exchange is the caller's (fastecc_b200/sharded.py does it

@@ -48,6 +48,13 @@ for N, M, S in ((3 << 10, 3 << 6, 1022), (1 << 12, 1 << 12, 16)):         # repa
     par[lost_p, :S] = -1
     fe.rs_repair_dev(data[:, :S], par[:, :S], lost_d, lost_p)
     assert torch.equal(data, want_d) and torch.equal(par, want_p), ("repair", N, M, S)
+for B, N, M, S in ((37, 12, 4, 7), (5, 64, 16, 1022), (9, 18, 9, 33)):  # the batch encode: M < 8 and M >= 8, SIZE % 4 != 0
+    data = torch.randint(-(1 << 31), 1 << 31, (B, N, (S + 3) // 4 * 4), dtype=torch.int32, device="cuda")[..., :S]
+    par = fe.rs_encode_batch_dev(data, M=M)
+    for b in (0, B - 1):
+        one = data[b].clone()
+        fe.rs_encode_asym_mixed_dev(one, M)
+        assert torch.equal(par[b], one[:M]), ("batch", B, N, M, S, b)
 raw = torch.randint(0, 256, (64, 4096), dtype=torch.uint8, device="cuda")
 w = fe.bytes_to_gfp_dev(raw)
 assert bool((fe.gfp_to_bytes_dev(w, 1024) == raw).all())

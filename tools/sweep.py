@@ -5,7 +5,7 @@ calls.  Arrays below ~100 MB stay in the 126 MB L2 between calls (marked); the s
 Then recoding, decoding, the asymmetric encode, the encode of 3 * 2^k / 9 * 2^k blocks (`encode_mixed`, DESIGN 3e) and
 their encode into fewer parity blocks (`encode_asym_mixed`, DESIGN 3f; `--asym-mixed`: only these).  `--repair`: only the repair
 of a stored stripe against the 2N-row decoder (DESIGN 3g); `--update`, `--scrub`, `--scrub-degraded`, `--reconstruct`: only the update (3h),
-the scrub (3i), the degraded scrub (3j) or the degraded read (3k) lines.
+the scrub (3i), the degraded scrub (3j) or the degraded read (3k) lines; `--batch`: only the batch encode of small stripes (3l).
 Prints one JSON line per point."""
 import json
 import os
@@ -553,7 +553,60 @@ def reconstruct_sweep():
         torch.cuda.empty_cache()
 
 
+def batch_sweep():
+    """Encode of a batch of small stripes (fastecc_b200_rs_encode_batch, DESIGN 3l) at the common storage shapes, 4 KiB blocks, B
+    stripes of about 1 GiB of data in all, data and parity in separate stripe-major buffers.  The batch call: CUDA events around
+    `reps` back-to-back calls.  Its floors: memory, (N + M) * B * 4096 bytes at the data sheet's 3.35 TB/s; products, M * N * B *
+    1024 at the 1.7e12 products/s that update_parity_kernel measured (DESIGN 3h); the larger one binds.  Beside it, the
+    per-stripe path on the first `few` stripes: clone the stripe, rs_encode_asym_mixed_dev, copy the M parity rows out; timed
+    with events around the loop and scaled to B.  The two alternated twice (the lower figures).  Each line names the card and
+    its power limit, read in the same run."""
+    from bench import gpu_identity
+    fe.init(0)
+    card = gpu_identity(torch.cuda.current_device())
+    S, few = 1024, 300
+    for N, M in ((4, 2), (6, 3), (8, 4), (9, 3), (12, 4), (16, 4), (18, 3), (32, 8), (48, 16), (64, 16), (64, 64)):
+        B = (1 << 30) // (N * S * 4)
+        data = (torch.arange(B * N * S, device="cuda", dtype=torch.int64) * 2654435761 % P).to(torch.int32).view(B, N, S)
+        parity = torch.empty((B, M, S), dtype=torch.int32, device="cuda")
+        fe.rs_encode_batch_dev(data, parity)
+        torch.cuda.synchronize()
+        ok = all(torch.equal(parity[b], _encode_one(data[b], M)) for b in (0, B // 2, B - 1))
+        scratch = torch.empty((N, S), dtype=torch.int32, device="cuda")
+        out = torch.empty((few, M, S), dtype=torch.int32, device="cuda")
+
+        def per_stripe():
+            for b in range(few):
+                scratch.copy_(data[b])
+                fe.rs_encode_asym_mixed_dev(scratch, M)
+                out[b].copy_(scratch[:M])
+        runs, runs_per = [], []
+        for _ in range(2):
+            runs.append(timed(lambda: fe.rs_encode_batch_dev(data, parity), 10))
+            runs_per.append(timed(per_stripe, 2) * B / few)
+        ms, ms_per = min(runs), min(runs_per)
+        mem_ms = (N + M) * B * S * 4 / 3.35e12 * 1e3
+        prod_ms = M * N * B * S / 1.7e12 * 1e3
+        print(json.dumps({"op": "encode_batch", "N": N, "M": M, "B": B, "block_bytes": 4 * S, "ok": ok, "ms": round(ms, 4), "ms_runs": [round(v, 4) for v in runs],
+                          "memory_floor_ms": round(mem_ms, 4), "product_floor_ms_at_1.7e12": round(prod_ms, 4),
+                          "binds": "memory" if mem_ms >= prod_ms else "products", "fraction_of_binding_floor": round(max(mem_ms, prod_ms) / ms, 3),
+                          "GBps_data_plus_parity": round((N + M) * B * S * 4 / ms / 1e6, 1),
+                          "per_stripe_ms_scaled_to_B": round(ms_per, 2), "per_stripe_stripes_timed": few, "speedup": round(ms_per / ms, 1),
+                          "gpu": card["name"], "power_limit_w": card["power_limit_w"]}), flush=True)
+        del data, parity, scratch, out
+        torch.cuda.empty_cache()
+
+
+def _encode_one(x, M):
+    buf = x.clone()
+    fe.rs_encode_asym_mixed_dev(buf, M)
+    return buf[:M]
+
+
 if __name__ == "__main__":
+    if "--batch" in sys.argv:                                 # only the batch encode lines
+        batch_sweep()
+        sys.exit(0)
     if "--reconstruct" in sys.argv:                           # only the degraded read lines
         reconstruct_sweep()
         sys.exit(0)
