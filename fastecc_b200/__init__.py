@@ -75,6 +75,8 @@ def lib() -> ctypes.CDLL:
         L.fastecc_b200_rs_scrub_degraded.argtypes = [vp, vp, sz, vp, sz, sz, sz, ctypes.c_uint64, vp, vp, vp, vp, vp, vp]; L.fastecc_b200_rs_scrub_degraded.restype = ci
         L.fastecc_b200_rs_reconstruct.argtypes = [vp, sz, sz, vp, sz, sz, vp, sz, vp, sz, vp, sz, vp, sz, vp, sz, sz, vp]; L.fastecc_b200_rs_reconstruct.restype = ci
         L.fastecc_b200_rs_encode_batch.argtypes = [vp, sz, sz, sz, vp, sz, sz, sz, sz, sz, vp]; L.fastecc_b200_rs_encode_batch.restype = ci
+        L.fastecc_b200_rs_reconstruct_batch.argtypes = [vp, sz, sz, sz, vp, sz, sz, sz, vp, sz, vp, sz, vp, sz, vp, sz, vp, sz, sz, sz, sz, vp]
+        L.fastecc_b200_rs_reconstruct_batch.restype = ci
         L.fastecc_b200_rs_encode_shard_pass.argtypes = [vp, sz, ci, ci, sz, sz, ci, vp]; L.fastecc_b200_rs_encode_shard_pass.restype = ci
         L.fastecc_b200_rs_encode_shard_pass_p2p.argtypes = [vp, vp, sz, ci, ci, sz, sz, ci, vp]; L.fastecc_b200_rs_encode_shard_pass_p2p.restype = ci
         L.fastecc_b200_ntt_shard_pass_p2p.argtypes = [vp, vp, sz, ci, ci, sz, sz, ci, ci, vp]; L.fastecc_b200_ntt_shard_pass_p2p.restype = ci
@@ -357,6 +359,14 @@ def rs_reconstruct_dev(data, parity, lost_data, lost_parity, want_data=None, wan
     return out
 
 
+def _batch_args(t, name):
+    """(pointer, B, rows, S, pitch, stripe stride) of a [B, rows, S] batch view"""
+    import torch
+    if not (t.is_cuda and t.dim() == 3 and t.dtype in (torch.int32, torch.uint32) and t.stride(2) == 1):
+        raise ValueError("%s: expected a 3-D CUDA int32/uint32 tensor with unit stride along the word dimension" % name)
+    return t.data_ptr(), t.shape[0], t.shape[1], t.shape[2], t.stride(1), t.stride(0)
+
+
 def rs_encode_batch_dev(data, parity=None, M=None):
     """Encode a batch of small stripes in one launch (fastecc_b200_rs_encode_batch, DESIGN 3l): data = [B, N, S] CUDA int32/uint32
     tensor with unit word stride (a view such as buf[:, :N, :S] of a [B, N + M, pitch] buffer is fine), read only; N <= 64 in the
@@ -365,11 +375,7 @@ def rs_encode_batch_dev(data, parity=None, M=None):
     allocated.  Rows 16-byte aligned with pitches and stripe strides that are multiples of 4 words; the parity may not overlap
     itself or the data.  Returns `parity`.  Asynchronous on the current stream."""
     import torch
-
-    def args(t, name):
-        if not (t.is_cuda and t.dim() == 3 and t.dtype in (torch.int32, torch.uint32) and t.stride(2) == 1):
-            raise ValueError("%s: expected a 3-D CUDA int32/uint32 tensor with unit stride along the word dimension" % name)
-        return t.data_ptr(), t.shape[0], t.shape[1], t.shape[2], t.stride(1), t.stride(0)
+    args = _batch_args
     dp, B, N, S, dpitch, dstride = args(data, "data")
     if parity is None:
         if M is None:
@@ -380,6 +386,37 @@ def rs_encode_batch_dev(data, parity=None, M=None):
         raise ValueError("parity is %d x %d x %d words for %d stripes of %s x %d-word blocks" % (pB, pM, pS, B, "M" if M is None else int(M), S))
     _check(lib().fastecc_b200_rs_encode_batch(dp, dpitch, dstride, N, pp, ppitch, pstride, pM, B, S, torch.cuda.current_stream(data.device).cuda_stream))
     return parity
+
+
+def rs_reconstruct_batch_dev(data, parity, lost_data, lost_parity, want_data=None, want_parity=None, out=None):
+    """Degraded read of a batch of small stripes with one loss pattern (fastecc_b200_rs_reconstruct_batch, DESIGN 3m): data =
+    [B, N, S], parity = [B, M, S] CUDA int32/uint32 tensors with unit word stride (views such as buf[:, :N, :S] are fine), read
+    only; N <= 64 in the family rs_encode_asym_mixed_dev accepts.  lost_data / lost_parity = the blocks every stripe lost (at most
+    M in all); want_data / want_parity = the lost blocks to produce (default: all of them).  Reads each stripe's surviving data
+    rows and its len(lost_data) lowest surviving parity rows only.  out = [B, n_out, S] receives each stripe's wanted data blocks,
+    then its wanted parity blocks, bit for bit what rs_reconstruct_dev gives for that stripe; when it is None, a new int32 tensor
+    with rows of ceil4(S) words is allocated.  Rows 16-byte aligned with pitches and stripe strides that are multiples of 4 words;
+    `out` may not overlap itself, the data or the parity.  Returns `out`.  Asynchronous on the current stream."""
+    import torch
+    from .decoder import _CPattern
+    dp, B, N, S, dpitch, dstride = _batch_args(data, "data")
+    pp, pB, M, pS, ppitch, pstride = _batch_args(parity, "parity")
+    if (pB, pS) != (B, S):
+        raise ValueError("parity is %d x %d x %d words for %d stripes of %d-word blocks" % (pB, M, pS, B, S))
+    u32 = lambda v: _CPattern._u32(v, "block numbers in [0, 2^32)")
+    ld, lp = u32(lost_data), u32(lost_parity)
+    wd = ld if want_data is None else u32(want_data)
+    wp = lp if want_parity is None else u32(want_parity)
+    n = wd.size + wp.size
+    if out is None:
+        out = torch.empty((B, n, (S + 3) // 4 * 4), dtype=torch.int32, device=data.device)[..., :S]
+    op, oB, on, oS, opitch, ostride = _batch_args(out, "out")
+    if (oB, on, oS) != (B, n, S):
+        raise ValueError("out is %d x %d x %d words for %d stripes of %d wanted blocks of %d words" % (oB, on, oS, B, n, S))
+    arr = lambda a: a.ctypes.data if a.size else None
+    _check(lib().fastecc_b200_rs_reconstruct_batch(dp, dpitch, dstride, N, pp, ppitch, pstride, M, arr(ld), ld.size, arr(lp), lp.size, arr(wd), wd.size,
+                                                   arr(wp), wp.size, op, opitch, ostride, B, S, torch.cuda.current_stream(data.device).cuda_stream))
+    return out
 
 
 def bytes_to_gfp_dev(raw, words=None):

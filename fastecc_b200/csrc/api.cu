@@ -732,7 +732,43 @@ int scrub_degraded(Context* c, const fastecc_b200_repair* R, const uint32_t* dat
     return 0;
 }
 
-// The combination of a degraded read (DESIGN 3k), n_out x a Barrett triples, row q for output q.  pos = J (a parity blocks) then the
+// x[i] = -2 / x[i] mod P for every i (all nonzero), by one batch inversion.
+void neg2_over(std::vector<uint32_t>& x)
+{
+    using gf::mulmod;
+    std::vector<uint32_t> pre(x.size() + 1, 1u);
+    for (size_t i = 0; i < x.size(); ++i) pre[i + 1] = mulmod(pre[i], x[i]);
+    uint32_t inv = gf::inv(pre[x.size()]);
+    for (size_t i = x.size(); i-- > 0;) {
+        const uint32_t t = mulmod(inv, pre[i]);
+        inv = mulmod(inv, x[i]);
+        x[i] = mulmod(gf::P - 2, t);
+    }
+}
+
+// The N entries of fastecc_b200_rs_update's table as plain words: T[t] = -2 / (N (rho^(2t+1) - 1)), rho = GF_Root(2N), equal to
+// update_table_kernel's canonical entries.
+std::vector<uint32_t> update_entries(size_t N)
+{
+    const uint32_t rho = gf::root((uint32_t)(2 * N)), n = (uint32_t)(N % gf::P);
+    std::vector<uint32_t> T(N);
+    for (size_t t = 0; t < N; ++t) T[t] = gf::mulmod(n, gf::sub(gf::powmod(rho, 2 * t + 1), 1u));
+    neg2_over(T);
+    return T;
+}
+
+// J of a degraded read (DESIGN 3k): the a lowest-numbered parity blocks not in lost_p (ascending, nlp of them, a + nlp <= M).
+std::vector<uint32_t> parity_rows_J(size_t a, const uint32_t* lost_p, size_t nlp)
+{
+    std::vector<uint32_t> J;
+    for (uint32_t j = 0, q = 0; J.size() < a; ++j) {
+        while (q < nlp && lost_p[q] < j) ++q;
+        if (q == nlp || lost_p[q] != j) J.push_back(j);
+    }
+    return J;
+}
+
+// The combination of a degraded read (DESIGN 3k), n_out x a plain words, row q for output q.  pos = J (a parity blocks) then the
 // wanted parity blocks; E = the a lost data blocks.  T(j, e) = T[(D j - e) mod N] = -2 / (N (y_j z_e - 1)), y_j = rho^(2 D j + 1),
 // z_e = rho^-2e, rho = GF_Root(2N), equals update_table_kernel's canonical entry (one batch inversion for all of them).  A = T(J, E)
 // is a Cauchy matrix up to diagonal scalings (the points y_j and z_e^-1 are distinct), so Gauss-Jordan always finds a pivot.
@@ -743,19 +779,13 @@ std::vector<uint32_t> reconstruct_combination(size_t N, size_t D, const std::vec
     using gf::mulmod;
     const size_t nk = pos.size();
     const uint32_t rho = gf::root((uint32_t)(2 * N)), n = (uint32_t)(N % gf::P);
-    std::vector<uint32_t> z(a), Tv(nk * a), pre(nk * a + 1, 1u);
+    std::vector<uint32_t> z(a), Tv(nk * a);
     for (size_t e = 0; e < a; ++e) z[e] = gf::powmod(rho, (2 * N - 2 * (uint64_t)E[e]) % (2 * N));
     for (size_t k = 0; k < nk; ++k) {
         const uint32_t y = gf::powmod(rho, 2 * D * (uint64_t)pos[k] + 1);
         for (size_t e = 0; e < a; ++e) Tv[k * a + e] = mulmod(n, gf::sub(mulmod(y, z[e]), 1u));
     }
-    for (size_t i = 0; i < nk * a; ++i) pre[i + 1] = mulmod(pre[i], Tv[i]);
-    uint32_t inv = gf::inv(pre[nk * a]);
-    for (size_t i = nk * a; i-- > 0;) {
-        const uint32_t t = mulmod(inv, pre[i]);
-        inv = mulmod(inv, Tv[i]);
-        Tv[i] = mulmod(gf::P - 2, t);
-    }
+    neg2_over(Tv);
     std::vector<uint32_t> A(Tv.begin(), Tv.begin() + a * a), X(a * a, 0u);  // [A | X], X from I to A^-1
     for (size_t i = 0; i < a; ++i) X[i * a + i] = 1;
     for (size_t col = 0; col < a; ++col) {
@@ -773,19 +803,29 @@ std::vector<uint32_t> reconstruct_combination(size_t N, size_t D, const std::vec
             }
         }
     }
-    std::vector<uint32_t> B((nwd + nwp) * a * 4);
-    auto put = [&](size_t q, size_t j, uint32_t w) { const gf::Tw t = gf::make_tw(w); uint32_t* b = &B[(q * a + j) * 4]; b[0] = t.w; b[1] = t.whi; b[2] = t.wlo; b[3] = 0; };
+    std::vector<uint32_t> B((nwd + nwp) * a);
     for (size_t q = 0, k = 0; q < nwd; ++q) {
         while (E[k] != want_d[q]) ++k;
-        for (size_t j = 0; j < a; ++j) put(q, j, X[k * a + j]);
+        for (size_t j = 0; j < a; ++j) B[q * a + j] = X[k * a + j];
     }
     for (size_t m = 0; m < nwp; ++m)
         for (size_t j = 0; j < a; ++j) {
             uint64_t s = 0;
             for (size_t k = 0; k < a; ++k) s += mulmod(Tv[(a + m) * a + k], X[k * a + j]);
-            put(nwd + m, j, (uint32_t)(s % gf::P));
+            B[(nwd + m) * a + j] = (uint32_t)(s % gf::P);
         }
     return B;
+}
+
+// Plain words as the Barrett triples {w, whi, wlo, 0} that gf::mul takes.
+std::vector<uint32_t> barrett_triples(const std::vector<uint32_t>& w)
+{
+    std::vector<uint32_t> t(w.size() * 4);
+    for (size_t i = 0; i < w.size(); ++i) {
+        const gf::Tw x = gf::make_tw(w[i]);
+        t[4 * i] = x.w; t[4 * i + 1] = x.whi; t[4 * i + 2] = x.wlo; t[4 * i + 3] = 0;
+    }
+    return t;
 }
 
 // The degraded read of one stripe (DESIGN 3k) on the repair workspace: K = a + nwp rows of 64-bit sums of one column chunk, then
@@ -794,14 +834,10 @@ int reconstruct(Context* c, const uint32_t* data, size_t dpitch, size_t N, const
                 size_t a, const uint32_t* lost_p, size_t nlp, const uint32_t* want_d, size_t nwd, const uint32_t* want_p, size_t nwp, uint32_t* out,
                 size_t opitch, size_t size, cudaStream_t st)
 {
-    std::vector<uint32_t> pos;                                      // J: the a lowest surviving parity blocks, then the wanted ones
-    for (uint32_t j = 0, q = 0; pos.size() < a; ++j) {
-        while (q < nlp && lost_p[q] < j) ++q;
-        if (q == nlp || lost_p[q] != j) pos.push_back(j);
-    }
+    std::vector<uint32_t> pos = parity_rows_J(a, lost_p, nlp);       // J, then the wanted parity blocks
     pos.insert(pos.end(), want_p, want_p + nwp);
     const size_t nk = pos.size(), n_out = nwd + nwp, D = N / M;
-    std::vector<uint32_t> up = reconstruct_combination(N, D, pos, lost_d, a, want_d, nwd, nwp);
+    std::vector<uint32_t> up = barrett_triples(reconstruct_combination(N, D, pos, lost_d, a, want_d, nwd, nwp));
     const size_t nb = up.size();
     up.insert(up.end(), pos.begin(), pos.end());
     up.insert(up.end(), lost_d, lost_d + a);
@@ -821,6 +857,65 @@ int reconstruct(Context* c, const uint32_t* data, size_t dpitch, size_t N, const
         CUDA_TRY(launch_reconstruct_sum(data + c0, dpitch, N, D, T, d_pos, nk, d_lost, a, cols, sums, c->num_sms, st)); g_launches++;
         CUDA_TRY(launch_reconstruct_combine(sums, parity + c0, ppitch, d_pos, a, B, n_out, nwd, out + c0, opitch, cols, c->num_sms, st)); g_launches++;
     }
+    return 0;
+}
+
+// The block lists of a degraded read, host arrays: non-null where not empty; lost and wanted blocks ascending, distinct and below N
+// or M; the wanted ones among the lost ones; at most M lost blocks in all.
+int check_reconstruct_lists(size_t N, size_t M, const uint32_t* lost_data, size_t n_lost_data, const uint32_t* lost_parity, size_t n_lost_parity,
+                            const uint32_t* want_data, size_t n_want_data, const uint32_t* want_parity, size_t n_want_parity, const char* who)
+{
+    if ((n_lost_data && !lost_data) || (n_lost_parity && !lost_parity) || (n_want_data && !want_data) || (n_want_parity && !want_parity))
+        return fail(FASTECC_B200_EINVAL, "%s: null block list", who);
+    if (!ascending_below(lost_data, n_lost_data, N) || !ascending_below(want_data, n_want_data, N))
+        return fail(FASTECC_B200_EINVAL, "%s: lost and wanted data blocks must be ascending, distinct and below N=%zu", who, N);
+    if (!ascending_below(lost_parity, n_lost_parity, M) || !ascending_below(want_parity, n_want_parity, M))
+        return fail(FASTECC_B200_EINVAL, "%s: lost and wanted parity blocks must be ascending, distinct and below M=%zu", who, M);
+    if (!std::includes(lost_data, lost_data + n_lost_data, want_data, want_data + n_want_data) ||
+        !std::includes(lost_parity, lost_parity + n_lost_parity, want_parity, want_parity + n_want_parity))
+        return fail(FASTECC_B200_EINVAL, "%s: every wanted block must be a lost one", who);
+    if (n_lost_data + n_lost_parity > M)
+        return fail(FASTECC_B200_EINVAL, "%s: %zu + %zu lost blocks exceed M=%zu", who, n_lost_data, n_lost_parity, M);
+    return 0;
+}
+
+// The degraded read of a batch of stripes with one loss pattern (DESIGN 3m).  The combination B of 3k folded into C, n_out x N over
+// the sources (the N - a surviving data rows ascending, then J): on surviving data row i, [q is parity block w] T(w, i) -
+// sum_j B[q][j] T(J_j, i); on parity row J_j, B[q][j]; T(j, i) = T[(D j - i) mod N].  C as triples, then the N source rows,
+// uploaded under repair's lease; one launch.
+int reconstruct_batch(Context* c, const uint32_t* data, size_t dpitch, size_t dstride, size_t N, const uint32_t* parity, size_t ppitch, size_t pstride,
+                      size_t M, const uint32_t* lost_d, size_t a, const uint32_t* lost_p, size_t nlp, const uint32_t* want_d, size_t nwd,
+                      const uint32_t* want_p, size_t nwp, uint32_t* out, size_t opitch, size_t ostride, size_t n_stripes, size_t size, cudaStream_t st)
+{
+    const size_t D = N / M, n_out = nwd + nwp, nd = N - a;
+    std::vector<uint32_t> pos = parity_rows_J(a, lost_p, nlp);       // J, then the wanted parity blocks
+    pos.insert(pos.end(), want_p, want_p + nwp);
+    const std::vector<uint32_t> B = reconstruct_combination(N, D, pos, lost_d, a, want_d, nwd, nwp), T = update_entries(N);
+    std::vector<uint32_t> src;
+    for (uint32_t i = 0, k = 0; i < N; ++i) {
+        if (k < a && lost_d[k] == i) ++k;
+        else src.push_back(i);
+    }
+    src.insert(src.end(), pos.begin(), pos.begin() + a);
+    const auto Tji = [&](size_t j, size_t i) { return T[(D * j + N - i) % N]; };
+    std::vector<uint32_t> C(n_out * N);
+    for (size_t q = 0; q < n_out; ++q) {
+        for (size_t s = 0; s < nd; ++s) {
+            uint64_t v = q >= nwd ? Tji(want_p[q - nwd], src[s]) : 0;
+            for (size_t j = 0; j < a; ++j) v += gf::P - gf::mulmod(B[q * a + j], Tji(pos[j], src[s]));
+            C[q * N + s] = (uint32_t)(v % gf::P);
+        }
+        for (size_t j = 0; j < a; ++j) C[q * N + nd + j] = B[q * a + j];
+    }
+    std::vector<uint32_t> up = barrett_triples(C);
+    const size_t nc = up.size();
+    up.insert(up.end(), src.begin(), src.end());
+    Lease ws(&c->repair, st);
+    CUDA_TRY(ws.acquire(up.size() * sizeof(uint32_t)));
+    uint32_t* d_up = ws.ptr();
+    TRY_RC(upload_list(c, up.data(), up.size(), d_up, st));
+    CUDA_TRY(launch_batch_reconstruct(data, dpitch, dstride, parity, ppitch, pstride, N, nd, (const uint4*)d_up, d_up + nc, n_out, out, opitch, ostride,
+                                      n_stripes, size, c->num_sms, st)); g_launches++;
     return 0;
 }
 
@@ -1157,17 +1252,9 @@ int fastecc_b200_rs_reconstruct(const uint32_t* d_data, size_t data_pitch, size_
     if (int rc = check_order(N, M, size, padded_pitch(size), FASTECC_B200_MAX_LOG_N_ENCODE, true, who)) return rc;
     if (int rc = check_rows(d_data, N, size, data_pitch, true, who)) return rc;
     if (int rc = check_rows(d_parity, M, size, parity_pitch, true, who)) return rc;
-    if ((n_lost_data && !lost_data) || (n_lost_parity && !lost_parity) || (n_want_data && !want_data) || (n_want_parity && !want_parity))
-        return fail(FASTECC_B200_EINVAL, "%s: null block list", who);
-    if (!ascending_below(lost_data, n_lost_data, N) || !ascending_below(want_data, n_want_data, N))
-        return fail(FASTECC_B200_EINVAL, "%s: lost and wanted data blocks must be ascending, distinct and below N=%zu", who, N);
-    if (!ascending_below(lost_parity, n_lost_parity, M) || !ascending_below(want_parity, n_want_parity, M))
-        return fail(FASTECC_B200_EINVAL, "%s: lost and wanted parity blocks must be ascending, distinct and below M=%zu", who, M);
-    if (!std::includes(lost_data, lost_data + n_lost_data, want_data, want_data + n_want_data) ||
-        !std::includes(lost_parity, lost_parity + n_lost_parity, want_parity, want_parity + n_want_parity))
-        return fail(FASTECC_B200_EINVAL, "%s: every wanted block must be a lost one", who);
-    if (n_lost_data + n_lost_parity > M)
-        return fail(FASTECC_B200_EINVAL, "%s: %zu + %zu lost blocks exceed M=%zu", who, n_lost_data, n_lost_parity, M);
+    if (int rc = check_reconstruct_lists(N, M, lost_data, n_lost_data, lost_parity, n_lost_parity, want_data, n_want_data, want_parity, n_want_parity,
+                                         who))
+        return rc;
     if (n_lost_data + n_want_parity > FASTECC_B200_RECONSTRUCT_MAX)
         return fail(FASTECC_B200_EINVAL, "%s: n_lost_data + n_want_parity = %zu exceeds FASTECC_B200_RECONSTRUCT_MAX = %d; fastecc_b200_rs_repair rebuilds up "
                     "to M lost blocks", who, n_lost_data + n_want_parity, FASTECC_B200_RECONSTRUCT_MAX);
@@ -1207,6 +1294,43 @@ int fastecc_b200_rs_encode_batch(const uint32_t* d_data, size_t data_pitch, size
     TRY_RC(update_table(c, N, st, &T));
     CUDA_TRY(launch_batch_encode(d_data, data_pitch, data_stride, N, d_parity, parity_pitch, parity_stride, M, n_stripes, size, T, st)); g_launches++;
     return 0;
+}
+
+int fastecc_b200_rs_reconstruct_batch(const uint32_t* d_data, size_t data_pitch, size_t data_stride, size_t N, const uint32_t* d_parity,
+                                      size_t parity_pitch, size_t parity_stride, size_t M, const uint32_t* lost_data, size_t n_lost_data,
+                                      const uint32_t* lost_parity, size_t n_lost_parity, const uint32_t* want_data, size_t n_want_data,
+                                      const uint32_t* want_parity, size_t n_want_parity, uint32_t* d_out, size_t out_pitch, size_t out_stride,
+                                      size_t n_stripes, size_t size, void* stream)
+{
+    const char* who = "fastecc_b200_rs_reconstruct_batch";
+    Context* c = ctx(who);
+    if (!c) return FASTECC_B200_ENOINIT;
+    if (int rc = check_order(N, M, size, padded_pitch(size), FASTECC_B200_MAX_LOG_N_ENCODE, true, who)) return rc;
+    if (N > FASTECC_B200_BATCH_MAX_N)
+        return fail(FASTECC_B200_EINVAL, "%s: N=%zu exceeds FASTECC_B200_BATCH_MAX_N = %d; read larger stripes one at a time with "
+                    "fastecc_b200_rs_reconstruct", who, N, FASTECC_B200_BATCH_MAX_N);
+    if (data_pitch < size || parity_pitch < size || out_pitch < size)
+        return fail(FASTECC_B200_EINVAL, "%s: needs SIZE_words (%zu) <= data_pitch_words (%zu), parity_pitch_words (%zu) and out_pitch_words (%zu)", who, size,
+                    data_pitch, parity_pitch, out_pitch);
+    if ((uintptr_t)d_data % 16 || (uintptr_t)d_parity % 16 || (uintptr_t)d_out % 16 || data_pitch % 4 || parity_pitch % 4 || out_pitch % 4 ||
+        data_stride % 4 || parity_stride % 4 || out_stride % 4)
+        return fail(FASTECC_B200_EINVAL, "%s: needs 16-byte aligned buffers and pitches and stripe strides that are multiples of 4 words", who);
+    if (int rc = check_reconstruct_lists(N, M, lost_data, n_lost_data, lost_parity, n_lost_parity, want_data, n_want_data, want_parity, n_want_parity,
+                                         who))
+        return rc;
+    const size_t n_out = n_want_data + n_want_parity;
+    if (!n_stripes || !n_out) return 0;                                   // nothing to read or write: any pointers do
+    if (!d_data || !d_parity || !d_out) return fail(FASTECC_B200_EINVAL, "%s: null device pointer", who);
+    if ((unsigned long long)n_stripes * ((size + 3) / 4) >= (1ull << 36))
+        return fail(FASTECC_B200_EINVAL, "%s: %zu stripes of %zu words exceed 2^36 16-byte chunks", who, n_stripes, size);
+    const BatchRows d{(uintptr_t)d_data / 4, data_pitch, data_stride, N}, p{(uintptr_t)d_parity / 4, parity_pitch, parity_stride, M};
+    const BatchRows o{(uintptr_t)d_out / 4, out_pitch, out_stride, n_out};
+    if (!batch_layout_disjoint(d, o, n_stripes, size) || !batch_layout_disjoint(p, o, n_stripes, size))
+        return fail(FASTECC_B200_EINVAL, "%s: output rows may overlap each other, the data or the parity; accepted layouts: an output span apart from "
+                    "each side's span, stripe-major or block-major, or one common stripe stride holding each stripe's rows disjoint", who);
+    return reconstruct_batch(c, d_data, data_pitch, data_stride, N, d_parity, parity_pitch, parity_stride, M, lost_data, n_lost_data, lost_parity,
+                             n_lost_parity, want_data, n_want_data, want_parity, n_want_parity, d_out, out_pitch, out_stride, n_stripes, size,
+                             (cudaStream_t)stream);
 }
 
 int fastecc_b200_pin_host_buffers(int enable)

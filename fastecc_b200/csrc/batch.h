@@ -1,6 +1,7 @@
-// Encode of a batch of small stripes (include/fastecc_b200.h: fastecc_b200_rs_encode_batch, DESIGN 3l): the layout rule that
-// decides, in O(N + M) host work, whether the parity rows of a batch are provably disjoint from each other and from the data,
-// and the one kernel launch.  The rule is plain C++ so that a host build can check it against brute-force word sets.
+// Encode and degraded read of a batch of small stripes (include/fastecc_b200.h: fastecc_b200_rs_encode_batch, DESIGN 3l, and
+// fastecc_b200_rs_reconstruct_batch, DESIGN 3m): the layout rule that decides, in O(N + M) host work, whether the rows a batch
+// writes are provably disjoint from each other and from the rows it reads, and the one kernel launch of each call.  The rule is
+// plain C++ so that a host build can check it against brute-force word sets.
 #pragma once
 #include <stdint.h>
 
@@ -69,5 +70,11 @@ namespace fecc {
 // One launch.
 cudaError_t launch_batch_encode(const uint32_t* data, size_t dpitch, size_t dstride, size_t N, uint32_t* parity, size_t ppitch, size_t pstride,
                                 size_t M, size_t B, size_t size, const uint4* T, cudaStream_t st);
+// Output row q < n_out of stripe b = sum_{s < N} C[q N + s] * source row s of stripe b, words [0, size) only, canonical; source
+// row s is data row src[s] for s < nd and parity row src[s] after (C and src on the device, C as Barrett triples {w, whi, wlo, 0},
+// n_out <= 64).  Source words are taken mod P; nothing else is read.  One launch of as many CTAs as fit on the SMs.
+cudaError_t launch_batch_reconstruct(const uint32_t* data, size_t dpitch, size_t dstride, const uint32_t* parity, size_t ppitch, size_t pstride,
+                                     size_t N, size_t nd, const uint4* C, const uint32_t* src, size_t n_out, uint32_t* out, size_t opitch,
+                                     size_t ostride, size_t B, size_t size, int num_sms, cudaStream_t st);
 }
 #endif

@@ -312,6 +312,41 @@ int fastecc_b200_rs_encode_batch(const uint32_t* d_data, size_t data_pitch_words
                                  uint32_t* d_parity, size_t parity_pitch_words, size_t parity_stripe_words, size_t M,
                                  size_t n_stripes, size_t SIZE_words, void* stream);
 
+/* ---- degraded read of a batch of small stripes with one loss pattern, in one launch -------------------------------------
+ * The read of many stripes that lost the same blocks (after a disk failure, the stripes that had the same block position on it):
+ * for each of n_stripes stripes, the wanted lost blocks into rows of their own; nothing is written into the stripes.  Stripes are
+ * addressed as in fastecc_b200_rs_encode_batch: data block i of stripe b at d_data + b * data_stripe_words + i * data_pitch_words,
+ * parity block j at d_parity + b * parity_stripe_words + j * parity_pitch_words; N is any order that
+ * fastecc_b200_rs_encode_asym_mixed_dev accepts up to FASTECC_B200_BATCH_MAX_N, M any divisor of N (larger stripes go through
+ * fastecc_b200_rs_reconstruct one at a time).  Every wanted block is a fixed combination of N rows (DESIGN 3m), so the call is
+ * n_out x N products per word straight from the stored rows.
+ *   Lists:    as for fastecc_b200_rs_reconstruct, one set for the whole batch: HOST arrays, ascending, distinct, below N or M;
+ *             the wanted blocks a subset of the lost ones; with a = n_lost_data, a + n_lost_parity <= M.
+ *             FASTECC_B200_RECONSTRUCT_MAX does not apply: n_out = n_want_data + n_want_parity <= M <= 64.
+ *   Rows read: per stripe exactly the N - a surviving data rows and the parity rows J = the a lowest-numbered parity blocks not in
+ *             lost_parity.  No other row is loaded: lost rows and parity rows outside J may hold anything.  Words are taken mod
+ *             P; pad words past SIZE never enter a sum.
+ *   Out:      wanted block q of stripe b (want_data in order, then want_parity) at d_out + b * out_stripe_words + q * out_pitch_words;
+ *             words [0, SIZE) of those rows only, canonical, each bit for bit what fastecc_b200_rs_reconstruct returns for that
+ *             stripe alone.  Nothing else is written; the stripe buffers are never written.
+ *   Layout:   the three bases 16-byte aligned; the pitches and stripe strides multiples of 4 words; each pitch >= SIZE.  Data and
+ *             parity may overlap each other (both are only read).  No output word may be another output word, a data word or a
+ *             parity word; the call accepts only layouts that fastecc_b200_rs_encode_batch's rule proves so for (data, out) and for
+ *             (parity, out): an output span apart from each side's span, stripe-major ([B][n_out][pitch]) or block-major
+ *             ([n_out][B][pitch]); or one common stripe stride holding each stripe's rows disjoint within it (e.g. one
+ *             [B][N + M + n_out][pitch] buffer).  Writing into the stripes' own lost rows is EINVAL.
+ * PRECONDITION: the surviving blocks are consistent stripes, as for fastecc_b200_rs_reconstruct.
+ * Validated in full before anything is allocated or launched (EINVAL).  n_stripes == 0 or nothing wanted returns 0 and launches
+ * nothing (null buffers included).  Otherwise one kernel launch and one host-to-device copy of the n_out x N coefficients (at
+ * most 64 KiB, through the context's repair workspace); no table build.  Asynchronous on the stream, which it does not
+ * synchronise; the host lists may be freed as soon as the call returns. */
+int fastecc_b200_rs_reconstruct_batch(const uint32_t* d_data, size_t data_pitch_words, size_t data_stripe_words, size_t N,
+                                      const uint32_t* d_parity, size_t parity_pitch_words, size_t parity_stripe_words, size_t M,
+                                      const uint32_t* lost_data, size_t n_lost_data, const uint32_t* lost_parity, size_t n_lost_parity,
+                                      const uint32_t* want_data, size_t n_want_data, const uint32_t* want_parity, size_t n_want_parity,
+                                      uint32_t* d_out, size_t out_pitch_words, size_t out_stripe_words,
+                                      size_t n_stripes, size_t SIZE_words, void* stream);
+
 /* ---- one transform sharded over several GPUs (one process per GPU; BASELINE config 4) ---------------------------
  * Global block i = l*n_ranks + rank is local block l (data in, parity out).  An encode is: pass 0 on every rank,
  * all-to-all of whole blocks, pass 1, all-to-all, pass 2 -- the exchange is the caller's (fastecc_b200/sharded.py does it

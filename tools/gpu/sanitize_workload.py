@@ -55,6 +55,13 @@ for B, N, M, S in ((37, 12, 4, 7), (5, 64, 16, 1022), (9, 18, 9, 33)):  # the ba
         one = data[b].clone()
         fe.rs_encode_asym_mixed_dev(one, M)
         assert torch.equal(par[b], one[:M]), ("batch", B, N, M, S, b)
+for B, N, M, S, ld, lp in ((37, 12, 4, 7, [2, 11], [0]), (5, 64, 16, 1022, [0, 9, 63], [3, 15]), (9, 18, 9, 33, [], [1, 8]),
+                          (6, 9, 3, 5, [0, 4, 8], [])):   # the batched degraded read: M < 8 and M >= 8, SIZE % 4 != 0, a = 0 with wanted parity, a = M
+    data = torch.randint(-(1 << 31), 1 << 31, (B, N, (S + 3) // 4 * 4), dtype=torch.int32, device="cuda")[..., :S]
+    par = fe.rs_encode_batch_dev(data, M=M)
+    out = fe.rs_reconstruct_batch_dev(data, par, ld, lp)
+    for b in (0, B - 1):
+        assert torch.equal(out[b], fe.rs_reconstruct_dev(data[b], par[b], ld, lp)), ("reconstruct batch", B, N, M, S, b)
 raw = torch.randint(0, 256, (64, 4096), dtype=torch.uint8, device="cuda")
 w = fe.bytes_to_gfp_dev(raw)
 assert bool((fe.gfp_to_bytes_dev(w, 1024) == raw).all())

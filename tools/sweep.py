@@ -5,7 +5,8 @@ calls.  Arrays below ~100 MB stay in the 126 MB L2 between calls (marked); the s
 Then recoding, decoding, the asymmetric encode, the encode of 3 * 2^k / 9 * 2^k blocks (`encode_mixed`, DESIGN 3e) and
 their encode into fewer parity blocks (`encode_asym_mixed`, DESIGN 3f; `--asym-mixed`: only these).  `--repair`: only the repair
 of a stored stripe against the 2N-row decoder (DESIGN 3g); `--update`, `--scrub`, `--scrub-degraded`, `--reconstruct`: only the update (3h),
-the scrub (3i), the degraded scrub (3j) or the degraded read (3k) lines; `--batch`: only the batch encode of small stripes (3l).
+the scrub (3i), the degraded scrub (3j) or the degraded read (3k) lines; `--batch`: only the batch encode of small stripes (3l);
+`--reconstruct-batch`: only the degraded read of a batch of small stripes (3m).
 Prints one JSON line per point."""
 import json
 import os
@@ -597,6 +598,78 @@ def batch_sweep():
         torch.cuda.empty_cache()
 
 
+def reconstruct_batch_sweep():
+    """Degraded read of a batch of small stripes with one loss pattern (fastecc_b200_rs_reconstruct_batch, DESIGN 3m) at the shapes
+    of --batch, 4 KiB blocks, B stripes of about 1 GiB of data in all, data, parity and output in separate stripe-major buffers.
+    Loss cases: (i) one lost data block, (ii) one lost parity block, (iii) two lost data blocks, (iv) M lost data blocks, all
+    wanted.  The call: CUDA events around `reps` back-to-back calls, alternated twice with rs_encode_batch_dev of the same
+    stripes (the lower figures).  The kernel: its device time in a torch.profiler trace of the same calls, over the memory floor
+    ((N + n_out) * B * 4096 bytes at the data sheet's 3.35 TB/s) and the product floor (n_out * N * B * 1024 products at the
+    1.7e12 products/s of update_parity_kernel, DESIGN 3h); the larger one binds.  The per-stripe path: rs_reconstruct_dev of the
+    first `few` stripes, events around the loop, scaled to B (n/a where a + n_want_parity > 32).  "ok": the output of three
+    sampled stripes equals their original blocks.  Each line names the card and its power limit, read in the same run."""
+    from torch.profiler import ProfilerActivity, profile
+    from bench import gpu_identity
+    fe.init(0)
+    card = gpu_identity(torch.cuda.current_device())
+    S, few, reps = 1024, 300, 10
+    rng = np.random.default_rng(7)
+
+    def kernel_ms(fn):
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(reps):
+                fn()
+            torch.cuda.synchronize()
+        us = [e.device_time_total for e in prof.key_averages() if "batch_reconstruct_kernel" in e.key]
+        return sum(us) / 1000 / reps if us else float("nan")
+
+    for N, M in ((4, 2), (6, 3), (8, 4), (9, 3), (12, 4), (16, 4), (18, 3), (32, 8), (48, 16), (64, 16), (64, 64)):
+        B = (1 << 30) // (N * S * 4)
+        data = (torch.arange(B * N * S, device="cuda", dtype=torch.int64) * 2654435761 % P).to(torch.int32).view(B, N, S)
+        parity = torch.empty((B, M, S), dtype=torch.int32, device="cuda")
+        fe.rs_encode_batch_dev(data, parity)
+        cases = [("i", sorted(rng.choice(N, size=1, replace=False).tolist()), []), ("ii", [], [M - 1])]
+        if M >= 2:
+            cases.append(("iii", sorted(rng.choice(N, size=2, replace=False).tolist()), []))
+        cases.append(("iv", sorted(rng.choice(N, size=M, replace=False).tolist()), []))
+        for case, ld, lp in cases:
+            n_out = len(ld) + len(lp)
+            out = torch.empty((B, n_out, S), dtype=torch.int32, device="cuda")
+            fe.rs_reconstruct_batch_dev(data, parity, ld, lp, out=out)
+            torch.cuda.synchronize()
+            ok = all(torch.equal(out[b], torch.cat([data[b, ld], parity[b, lp]])) for b in (0, B // 2, B - 1))
+            call = lambda: fe.rs_reconstruct_batch_dev(data, parity, ld, lp, out=out)
+            runs, runs_enc = [], []
+            for _ in range(2):
+                runs.append(timed(call, reps))
+                runs_enc.append(timed(lambda: fe.rs_encode_batch_dev(data, parity), reps))
+            k_ms = min(kernel_ms(call) for _ in range(2))
+            ms, ms_enc = min(runs), min(runs_enc)
+            per = None
+            if len(ld) + len(lp) <= 32:
+                one = torch.empty((few, n_out, S), dtype=torch.int32, device="cuda")
+
+                def per_stripe():
+                    for b in range(few):
+                        fe.rs_reconstruct_dev(data[b], parity[b], ld, lp, out=one[b])
+                per = min(timed(per_stripe, 2) for _ in range(2)) * B / few
+                del one
+            mem_ms = (N + n_out) * B * S * 4 / 3.35e12 * 1e3
+            prod_ms = n_out * N * B * S / 1.7e12 * 1e3
+            print(json.dumps({"op": "reconstruct_batch", "N": N, "M": M, "B": B, "case": case, "a": len(ld), "n_out": n_out, "block_bytes": 4 * S,
+                              "ok": ok, "call_ms": round(ms, 4), "call_ms_runs": [round(v, 4) for v in runs], "kernel_ms": round(k_ms, 4),
+                              "memory_floor_ms": round(mem_ms, 4), "product_floor_ms_at_1.7e12": round(prod_ms, 4),
+                              "binds": "memory" if mem_ms >= prod_ms else "products", "memory_floor_frac": round(mem_ms / k_ms, 3),
+                              "fraction_of_binding_floor": round(max(mem_ms, prod_ms) / k_ms, 3),
+                              "encode_batch_ms": round(ms_enc, 4), "vs_encode_batch": round(ms_enc / ms, 3),
+                              "per_stripe_ms_scaled_to_B": "n/a" if per is None else round(per, 2), "per_stripe_stripes_timed": few,
+                              "speedup_vs_per_stripe": "n/a" if per is None else round(per / ms, 1),
+                              "gpu": card["name"], "power_limit_w": card["power_limit_w"]}), flush=True)
+            del out
+        del data, parity
+        torch.cuda.empty_cache()
+
+
 def _encode_one(x, M):
     buf = x.clone()
     fe.rs_encode_asym_mixed_dev(buf, M)
@@ -604,6 +677,9 @@ def _encode_one(x, M):
 
 
 if __name__ == "__main__":
+    if "--reconstruct-batch" in sys.argv:                     # only the batched degraded read lines
+        reconstruct_batch_sweep()
+        sys.exit(0)
     if "--batch" in sys.argv:                                 # only the batch encode lines
         batch_sweep()
         sys.exit(0)
