@@ -77,6 +77,7 @@ def lib() -> ctypes.CDLL:
         L.fastecc_b200_rs_encode_batch.argtypes = [vp, sz, sz, sz, vp, sz, sz, sz, sz, sz, vp]; L.fastecc_b200_rs_encode_batch.restype = ci
         L.fastecc_b200_rs_reconstruct_batch.argtypes = [vp, sz, sz, sz, vp, sz, sz, sz, vp, sz, vp, sz, vp, sz, vp, sz, vp, sz, sz, sz, sz, vp]
         L.fastecc_b200_rs_reconstruct_batch.restype = ci
+        L.fastecc_b200_rs_update_batch.argtypes = [vp, sz, sz, sz, vp, sz, sz, sz, vp, sz, vp, sz, sz, sz, sz, vp]; L.fastecc_b200_rs_update_batch.restype = ci
         L.fastecc_b200_rs_encode_shard_pass.argtypes = [vp, sz, ci, ci, sz, sz, ci, vp]; L.fastecc_b200_rs_encode_shard_pass.restype = ci
         L.fastecc_b200_rs_encode_shard_pass_p2p.argtypes = [vp, vp, sz, ci, ci, sz, sz, ci, vp]; L.fastecc_b200_rs_encode_shard_pass_p2p.restype = ci
         L.fastecc_b200_ntt_shard_pass_p2p.argtypes = [vp, vp, sz, ci, ci, sz, sz, ci, ci, vp]; L.fastecc_b200_ntt_shard_pass_p2p.restype = ci
@@ -417,6 +418,28 @@ def rs_reconstruct_batch_dev(data, parity, lost_data, lost_parity, want_data=Non
     _check(lib().fastecc_b200_rs_reconstruct_batch(dp, dpitch, dstride, N, pp, ppitch, pstride, M, arr(ld), ld.size, arr(lp), lp.size, arr(wd), wd.size,
                                                    arr(wp), wp.size, op, opitch, ostride, B, S, torch.cuda.current_stream(data.device).cuda_stream))
     return out
+
+
+def rs_update_batch_dev(data, parity, changed, new) -> None:
+    """Update a batch of small stripes in place with one changed list (fastecc_b200_rs_update_batch, DESIGN 3n): data = [B, N, S],
+    parity = [B, M, S] and new = [B, k, S] CUDA int32/uint32 tensors with unit word stride (views such as buf[:, :N, :S] are
+    fine; new may be expanded over B with stride 0); N <= 64 in the family rs_encode_asym_mixed_dev accepts.  changed = k
+    ascending distinct block numbers below N, the same for every stripe; row q of new[b] is the new content of data block
+    changed[q] of stripe b.  The changed data rows receive their canonical new blocks and the parity becomes the batch encode of
+    the updated data; the stored parity must be the encode of the stored data.  Data rows outside `changed` are never read.  All
+    N + M rows of all stripes must be pairwise disjoint and apart from the new rows.  Asynchronous on the current stream."""
+    import torch
+    from .decoder import _CPattern
+    dp, B, N, S, dpitch, dstride = _batch_args(data, "data")
+    pp, pB, M, pS, ppitch, pstride = _batch_args(parity, "parity")
+    nptr, nB, k, nS, npitch, nstride = _batch_args(new, "new")
+    idx = _CPattern._u32(changed, "changed: block numbers in [0, 2^32)")
+    if k != idx.size:
+        raise ValueError("new has %d rows for %d changed blocks" % (k, idx.size))
+    if not (B == pB == nB and S == pS == nS):
+        raise ValueError("data, parity and new are %d x %d, %d x %d and %d x %d (stripes x words)" % (B, S, pB, pS, nB, nS))
+    _check(lib().fastecc_b200_rs_update_batch(dp, dpitch, dstride, N, pp, ppitch, pstride, M, idx.ctypes.data if idx.size else None, idx.size, nptr,
+                                              npitch, nstride, B, S, torch.cuda.current_stream(data.device).cuda_stream))
 
 
 def bytes_to_gfp_dev(raw, words=None):

@@ -1333,6 +1333,42 @@ int fastecc_b200_rs_reconstruct_batch(const uint32_t* d_data, size_t data_pitch,
                              (cudaStream_t)stream);
 }
 
+int fastecc_b200_rs_update_batch(uint32_t* d_data, size_t data_pitch, size_t data_stride, size_t N, uint32_t* d_parity, size_t parity_pitch,
+                                 size_t parity_stride, size_t M, const uint32_t* changed, size_t n_changed, const uint32_t* d_new, size_t new_pitch,
+                                 size_t new_stride, size_t n_stripes, size_t size, void* stream)
+{
+    const char* who = "fastecc_b200_rs_update_batch";
+    Context* c = ctx(who);
+    if (!c) return FASTECC_B200_ENOINIT;
+    if (int rc = check_order(N, M, size, padded_pitch(size), FASTECC_B200_MAX_LOG_N_ENCODE, true, who)) return rc;
+    if (N > FASTECC_B200_BATCH_MAX_N)
+        return fail(FASTECC_B200_EINVAL, "%s: N=%zu exceeds FASTECC_B200_BATCH_MAX_N = %d; update larger stripes one at a time with "
+                    "fastecc_b200_rs_update", who, N, FASTECC_B200_BATCH_MAX_N);
+    if (data_pitch < size || parity_pitch < size || new_pitch < size)
+        return fail(FASTECC_B200_EINVAL, "%s: needs SIZE_words (%zu) <= data_pitch_words (%zu), parity_pitch_words (%zu) and new_pitch_words (%zu)", who, size,
+                    data_pitch, parity_pitch, new_pitch);
+    if ((uintptr_t)d_data % 16 || (uintptr_t)d_parity % 16 || (uintptr_t)d_new % 16 || data_pitch % 4 || parity_pitch % 4 || new_pitch % 4 ||
+        data_stride % 4 || parity_stride % 4 || new_stride % 4)
+        return fail(FASTECC_B200_EINVAL, "%s: needs 16-byte aligned buffers and pitches and stripe strides that are multiples of 4 words", who);
+    if (n_changed && !changed) return fail(FASTECC_B200_EINVAL, "%s: null list of changed blocks", who);
+    if (!ascending_below(changed, n_changed, N)) return fail(FASTECC_B200_EINVAL, "%s: changed data blocks must be ascending, distinct and below N=%zu", who, N);
+    if (!n_stripes || !n_changed) return 0;                                // nothing to read or write: any pointers do
+    if (!d_data || !d_parity || !d_new) return fail(FASTECC_B200_EINVAL, "%s: null device pointer", who);
+    if ((unsigned long long)n_stripes * ((size + 3) / 4) >= (1ull << 36))
+        return fail(FASTECC_B200_EINVAL, "%s: %zu stripes of %zu words exceed 2^36 16-byte chunks", who, n_stripes, size);
+    const BatchRows d{(uintptr_t)d_data / 4, data_pitch, data_stride, N}, p{(uintptr_t)d_parity / 4, parity_pitch, parity_stride, M};
+    const BatchRows n{(uintptr_t)d_new / 4, new_pitch, new_stride, n_changed};
+    if (!batch_update_layout_disjoint(d, p, n, n_stripes, size))
+        return fail(FASTECC_B200_EINVAL, "%s: the data and parity rows of all stripes must be pairwise disjoint and apart from the new rows; accepted "
+                    "layouts: separate spans, each stripe-major or block-major, or one common stripe stride holding each stripe's rows disjoint", who);
+    const cudaStream_t st = (cudaStream_t)stream;
+    const uint4* T = nullptr;
+    TRY_RC(update_table(c, N, st, &T));
+    CUDA_TRY(launch_batch_update(d_data, data_pitch, data_stride, N, d_parity, parity_pitch, parity_stride, M, changed, n_changed, d_new, new_pitch,
+                                 new_stride, n_stripes, size, T, c->num_sms, st)); g_launches++;
+    return 0;
+}
+
 int fastecc_b200_pin_host_buffers(int enable)
 {
     std::lock_guard<std::mutex> lk(g_host_mu);

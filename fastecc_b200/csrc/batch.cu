@@ -322,3 +322,195 @@ cudaError_t launch_batch_reconstruct(const uint32_t* data, size_t dpitch, size_t
 }
 
 } // namespace fecc
+
+namespace {
+
+// Dynamic shared memory of batch_update_kernel's ring: with its 4.8 KiB of static arrays and the 1 KiB the SM reserves per CTA,
+// two CTAs fit in the 228 KiB of an SM
+constexpr uint32_t kUpdateRingBudget = 108 << 10;
+
+// Update of a batch in place with one changed list (fastecc_b200_rs_update_batch, DESIGN 3n): parity j of every stripe +=
+// sum_q (new_q - old_{e_q}) * T[(D j - e_q) mod N], and data row e_q := canon(new_q).  The skeleton of batch_reconstruct_kernel:
+// persistent CTAs walk tiles of items = 2^lg_items consecutive items through a ring of `stages` slots filled by 16-byte cp.async
+// (pad words zero-filled).  A tile holds rows = 2k + M rows: the k old changed data rows, the k new rows, then the M parity rows.
+// Once a tile has landed, thread t takes the flat (changed row, item) pairs t + 256 s: it stores the canonical new chunk into the
+// data row and leaves delta = subl(new, canon(old)) in the old row's slot, so every old word is in shared memory before it is
+// overwritten.  After a barrier the work units (group g of 32 items, outputs h + W v) start from the stored parity chunk, raw, add
+// delta times the broadcast triple from the T staged once per CTA with Barrett products and lazy sums (k M products per word), and
+// end with one canon and one store; with fewer than 8 units the k rows are split over `slices` warps as in the degraded read.  The
+// stripes are read through cp.async only (L2, never the non-coherent path), and nothing but words [0, SIZE) of the changed data
+// rows and the parity rows is written; the layout rule makes each written word one that only its own item reads.
+struct ChangedRows { uint32_t e[kMaxN]; };
+
+template <uint32_t U>
+__global__ void __launch_bounds__(256, 2) batch_update_kernel(uint32_t* data, size_t dpitch, size_t dstride, uint32_t N, uint32_t* parity,
+                                                              size_t ppitch, size_t pstride, uint32_t M, const uint32_t* nw, size_t npitch,
+                                                              size_t nstride, const ChangedRows ch, uint32_t k, const uint4* __restrict__ T,
+                                                              uint32_t W, uint32_t slices, uint32_t stages, uint32_t lg_items, uint32_t s4,
+                                                              double inv_s4, uint64_t n_items, uint64_t n_tiles, size_t size)
+{
+    extern __shared__ uint4 ring[];                                // [stage][row of the tile][item of the tile]
+    __shared__ uint4 stab[kMaxN];
+    __shared__ uint32_t se[kMaxN];
+    __shared__ uint4 spart[7 * 32];                                // partial sums of slices 1 .. 7: [slice - 1][unit][lane]
+    const uint32_t tid = threadIdx.x, lane = tid % 32, warp = tid / 32, items = 1u << lg_items, rows = 2 * k + M, chunks = rows << lg_items;
+    const uint32_t units = items / 32 * W, D = N / M, zero = gf::opaque_zero();
+    const uint4 z4 = make_uint4(0, 0, 0, 0);
+    if (tid < N) stab[tid] = __ldg(T + tid);
+    if (tid < k) se[tid] = ch.e[tid];
+    __syncthreads();
+
+    uint64_t next = blockIdx.x;                                    // the next tile to copy, into ring slot `put`
+    uint32_t put = 0;
+    auto issue = [&]() {
+        if (next < n_tiles) {
+            uint4* const slot = ring + (size_t)put * chunks;
+            const uint64_t tile = next;
+            for (uint32_t f = tid; f < chunks; f += 256) {
+                const uint32_t r = f >> lg_items;
+                const uint64_t it = (tile << lg_items) + (f & (items - 1));
+                if (it < n_items) {
+                    uint64_t b;
+                    uint32_t c;
+                    split_item(it, s4, inv_s4, b, c);
+                    const uint32_t* row = r < k ? data + b * dstride + se[r] * dpitch
+                                        : r < 2 * k ? nw + b * nstride + (r - k) * npitch : parity + b * pstride + (r - 2 * k) * ppitch;
+                    const size_t keep = size - 4 * (size_t)c;
+                    copy16_async(slot + f, row + 4 * (size_t)c, keep < 4 ? 4 * (uint32_t)keep : 16u);
+                } else {
+                    slot[f] = z4;
+                }
+            }
+        }
+        commit_async();
+        next += gridDim.x;
+        put = put + 1 == stages ? 0 : put + 1;
+    };
+    for (uint32_t s = 0; s + 1 < stages; ++s) issue();
+    for (uint64_t tile = blockIdx.x, get = 0; tile < n_tiles; tile += gridDim.x, get = get + 1 == stages ? 0 : get + 1) {
+        issue();                                                   // stages - 1 tiles ahead, into the slot consumed in the previous round
+        wait_async(stages - 1);
+        __syncthreads();                                           // this tile is in slot `get`
+        uint4* const sd = ring + (size_t)get * chunks;
+        for (uint32_t f = tid; f < k << lg_items; f += 256) {      // the new rows into the data, the deltas into the old rows' slots
+            const uint32_t q = f >> lg_items;
+            const uint64_t it = (tile << lg_items) + (f & (items - 1));
+            const uint4 o = gf::canon4(sd[f]), n = sd[f + (k << lg_items)];
+            sd[f] = make_uint4(gf::subl(n.x, o.x), gf::subl(n.y, o.y), gf::subl(n.z, o.z), gf::subl(n.w, o.w));
+            if (it >= n_items) continue;
+            uint64_t b;
+            uint32_t c;
+            split_item(it, s4, inv_s4, b, c);
+            uint32_t* dst = data + b * dstride + se[q] * dpitch + 4 * (size_t)c;
+            if (4 * (size_t)c + 4 <= size) __stcg(reinterpret_cast<uint4*>(dst), gf::canon4(n));
+            else store_row(dst, 0, gf::canon4(n), size - 4 * (size_t)c);
+        }
+        __syncthreads();                                           // every delta of the tile is in place
+        const uint32_t jobs = slices > 1 ? units * slices : units;
+        for (uint32_t u = warp; u < jobs; u += 8) {
+            const uint32_t unit = slices > 1 ? u % units : u, slice = slices > 1 ? u / units : 0;
+            const uint32_t g = unit / W, h = unit - g * W;
+            const uint4* col = sd + 32 * g + lane;
+            uint4 acc[U];
+            uint32_t base[U];
+#pragma unroll
+            for (uint32_t v = 0; v < U; ++v) {
+                const uint32_t j = h + W * v;
+                acc[v] = slice == 0 && j < M ? col[(2 * k + j) << lg_items] : z4;
+                base[v] = D * j + N;
+            }
+            for (uint32_t q = slice; q < k; q += slices) {
+                const uint4 d = col[q << lg_items];
+                const uint32_t e = se[q];
+#pragma unroll
+                for (uint32_t v = 0; v < U; ++v) {
+                    if (h + W * v >= M) continue;                  // the same for the whole warp
+                    uint32_t t = base[v] - e;
+                    if (t >= N) t -= N;
+                    const uint4 w = stab[t];
+                    acc[v].x = gf::addl(acc[v].x, gf::mul(d.x, w.x, w.y, w.z, zero));
+                    acc[v].y = gf::addl(acc[v].y, gf::mul(d.y, w.x, w.y, w.z, zero));
+                    acc[v].z = gf::addl(acc[v].z, gf::mul(d.z, w.x, w.y, w.z, zero));
+                    acc[v].w = gf::addl(acc[v].w, gf::mul(d.w, w.x, w.y, w.z, zero));
+                }
+            }
+            if (slices > 1) {                                      // U = 1 and one job per warp: slices 1 .. R - 1 hand their sums to slice 0
+                if (slice) {
+                    spart[((slice - 1) * units + unit) * 32 + lane] = gf::canon4(acc[0]);
+                    asm volatile("bar.arrive 1, %0;\n" ::"r"(32 * jobs) : "memory");
+                    continue;
+                }
+                asm volatile("bar.sync 1, %0;\n" ::"r"(32 * jobs) : "memory");
+                for (uint32_t s = 1; s < slices; ++s) {
+                    const uint4 p = spart[((s - 1) * units + unit) * 32 + lane];
+                    acc[0].x = gf::addl(acc[0].x, p.x);
+                    acc[0].y = gf::addl(acc[0].y, p.y);
+                    acc[0].z = gf::addl(acc[0].z, p.z);
+                    acc[0].w = gf::addl(acc[0].w, p.w);
+                }
+            }
+            const uint64_t it = (tile << lg_items) + 32 * g + lane;
+            if (it >= n_items) continue;
+            uint64_t b;
+            uint32_t c;
+            split_item(it, s4, inv_s4, b, c);
+            uint32_t* dst = parity + b * pstride + (size_t)ppitch * h + 4 * (size_t)c;
+            if (4 * (size_t)c + 4 <= size) {
+#pragma unroll
+                for (uint32_t v = 0; v < U; ++v)
+                    if (h + W * v < M) __stcg(reinterpret_cast<uint4*>(dst + (size_t)ppitch * W * v), gf::canon4(acc[v]));
+            } else {
+#pragma unroll
+                for (uint32_t v = 0; v < U; ++v)
+                    if (h + W * v < M) store_row(dst + (size_t)ppitch * W * v, 0, gf::canon4(acc[v]), size - 4 * (size_t)c);
+            }
+        }
+        __syncthreads();                                           // the slot (and spart) is consumed
+    }
+    wait_async(0);
+}
+
+} // namespace
+
+namespace fecc {
+
+cudaError_t launch_batch_update(uint32_t* data, size_t dpitch, size_t dstride, size_t N, uint32_t* parity, size_t ppitch, size_t pstride, size_t M,
+                                const uint32_t* changed, size_t k, const uint32_t* nw, size_t npitch, size_t nstride, size_t B, size_t size,
+                                const uint4* T, int num_sms, cudaStream_t st)
+{
+    const uint32_t U = M <= 8 ? 1 : M <= 16 ? 2 : M <= 24 ? 3 : M <= 32 ? 4 : M <= 48 ? 6 : 8;
+    const uint32_t W = (uint32_t)((M + U - 1) / U), rows = (uint32_t)(2 * k + M);
+    uint32_t lg_items = 5;                                         // the fewest items, a power of two, with a tile of >= 2048 chunks
+    while ((rows << lg_items) < kTileChunks) ++lg_items;
+    const uint32_t units = (1u << lg_items) / 32 * W, slices = U == 1 && units < 8 ? (uint32_t)std::min<size_t>(8 / units, k) : 1;
+    // Ring stages: as many tiles (up to 4) as fit in the shared memory of one of two CTAs per SM beside the static arrays, at least one
+    const size_t tile = ((size_t)rows << lg_items) * sizeof(uint4), budget = (size_t)kUpdateRingBudget;
+    const uint32_t stages = 2 * tile <= budget ? (uint32_t)std::min<size_t>(4, budget / tile) : 1;
+    const uint32_t s4 = (uint32_t)((size + 3) / 4);
+    const uint64_t n_items = (uint64_t)B * s4, n_tiles = (n_items + (1u << lg_items) - 1) >> lg_items;
+    const size_t smem = stages * tile;
+    ChangedRows ch{};
+    for (size_t q = 0; q < k; ++q) ch.e[q] = changed[q];
+    int per_sm = 0;
+#define BATCH_UPDATE(UU)                                                                                                                     \
+    do {                                                                                                                                     \
+        if (cudaError_t e = cudaFuncSetAttribute(batch_update_kernel<UU>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) return e;  \
+        if (cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, batch_update_kernel<UU>, 256, smem)) return e;            \
+        const uint64_t cap = (uint64_t)(per_sm > 1 ? per_sm : 1) * num_sms;                                                                  \
+        batch_update_kernel<UU><<<(unsigned)(n_tiles < cap ? n_tiles : cap), 256, smem, st>>>(                                                 \
+            data, dpitch, dstride, (uint32_t)N, parity, ppitch, pstride, (uint32_t)M, nw, npitch, nstride, ch, (uint32_t)k, T, W, slices, stages, \
+            lg_items, s4, 1.0 / s4, n_items, n_tiles, size);                                                                                 \
+    } while (0)
+    switch (U) {
+    case 1: BATCH_UPDATE(1); break;
+    case 2: BATCH_UPDATE(2); break;
+    case 3: BATCH_UPDATE(3); break;
+    case 4: BATCH_UPDATE(4); break;
+    case 6: BATCH_UPDATE(6); break;
+    default: BATCH_UPDATE(8); break;
+    }
+#undef BATCH_UPDATE
+    return cudaGetLastError();
+}
+
+} // namespace fecc

@@ -1,6 +1,7 @@
-// Encode and degraded read of a batch of small stripes (include/fastecc_b200.h: fastecc_b200_rs_encode_batch, DESIGN 3l, and
-// fastecc_b200_rs_reconstruct_batch, DESIGN 3m): the layout rule that decides, in O(N + M) host work, whether the rows a batch
-// writes are provably disjoint from each other and from the rows it reads, and the one kernel launch of each call.  The rule is
+// Encode, degraded read and update of a batch of small stripes (include/fastecc_b200.h: fastecc_b200_rs_encode_batch, DESIGN 3l,
+// fastecc_b200_rs_reconstruct_batch, DESIGN 3m, and fastecc_b200_rs_update_batch, DESIGN 3n): the layout rules that decide, in
+// O(N + M) host work, whether the rows a batch writes are provably disjoint from each other and from the rows it reads, and the
+// one kernel launch of each call.  The rule is
 // plain C++ so that a host build can check it against brute-force word sets.
 #pragma once
 #include <stdint.h>
@@ -60,6 +61,15 @@ inline bool batch_layout_disjoint(const BatchRows& d, const BatchRows& p, uint64
     return (d1 > p1 ? d1 : p1) - lo <= p.stride;
 }
 
+// The layout rule of fastecc_b200_rs_update_batch (DESIGN 3n), which writes into the stripes it reads: the rule above for the three
+// pairs (new, data), (new, parity) and (data, parity).  True only when all N + M rows of all stripes are pairwise disjoint and none
+// of them meets a new row (new rows may overlap each other: they are only read).  Then each word written, a changed data word or a
+// parity word, is read by the one work item that writes it and by no other, so an in-place write cannot feed another item's sum.
+inline bool batch_update_layout_disjoint(const BatchRows& d, const BatchRows& p, const BatchRows& n, uint64_t B, uint64_t size)
+{
+    return batch_layout_disjoint(n, d, B, size) && batch_layout_disjoint(n, p, B, size) && batch_layout_disjoint(d, p, B, size);
+}
+
 } // namespace fecc
 
 #if defined(__CUDACC__)
@@ -76,5 +86,13 @@ cudaError_t launch_batch_encode(const uint32_t* data, size_t dpitch, size_t dstr
 cudaError_t launch_batch_reconstruct(const uint32_t* data, size_t dpitch, size_t dstride, const uint32_t* parity, size_t ppitch, size_t pstride,
                                      size_t N, size_t nd, const uint4* C, const uint32_t* src, size_t n_out, uint32_t* out, size_t opitch,
                                      size_t ostride, size_t B, size_t size, int num_sms, cudaStream_t st);
+// In place, for B stripes with one host list changed[0 .. k) (ascending, below N <= 64): data row changed[q] of stripe b := the
+// canonical new row q of stripe b, and parity row j += sum_q (new_q - old_q) * T[(D j - changed[q]) mod N], words [0, size) only,
+// canonical; every word read is taken mod P.  Reads only the k changed data rows, the k new rows and the M parity rows; the list
+// goes by value in the launch's parameters.  Needs a layout batch_update_layout_disjoint accepts.  One launch of as many CTAs as
+// fit on the SMs.
+cudaError_t launch_batch_update(uint32_t* data, size_t dpitch, size_t dstride, size_t N, uint32_t* parity, size_t ppitch, size_t pstride, size_t M,
+                                const uint32_t* changed, size_t k, const uint32_t* nw, size_t npitch, size_t nstride, size_t B, size_t size,
+                                const uint4* T, int num_sms, cudaStream_t st);
 }
 #endif

@@ -347,6 +347,43 @@ int fastecc_b200_rs_reconstruct_batch(const uint32_t* d_data, size_t data_pitch_
                                       uint32_t* d_out, size_t out_pitch_words, size_t out_stripe_words,
                                       size_t n_stripes, size_t SIZE_words, void* stream);
 
+/* ---- update of a batch of small stripes in place with one changed list, in one launch -----------------------------------
+ * The partial write of many stripes at once: in each of n_stripes stripes the data blocks of one HOST list `changed` get new
+ * content and the M parity blocks are brought up to date, as fastecc_b200_rs_update does for one stripe (DESIGN 3n).  A caller
+ * groups its writes by the changed positions, as it groups degraded reads by loss pattern.  Data block i of stripe b is at
+ * d_data + b * data_stripe_words + i * data_pitch_words, parity block j at d_parity + b * parity_stripe_words + j * parity_pitch_words,
+ * and row q of stripe b's new rows, at d_new + b * new_stripe_words + q * new_pitch_words, is the new content of data block
+ * changed[q].  N is any order that fastecc_b200_rs_encode_asym_mixed_dev accepts up to FASTECC_B200_BATCH_MAX_N, M any divisor
+ * of N (larger stripes go through fastecc_b200_rs_update one at a time); changed is ascending, distinct, below N.
+ *   Result:  in every stripe data rows changed[q] hold the canonical new blocks and the M parity rows equal
+ *            fastecc_b200_rs_encode_batch (and so fastecc_b200_rs_encode_asym_mixed_dev) of the updated data, bit for bit.  The
+ *            change times update's table is added to the parity: n_changed x M products per word.
+ *   Writes:  words [0, SIZE) of the n_changed changed data rows and the M parity rows of each stripe, and nothing else: no other
+ *            data row, no pad word, no word between rows, never d_new.  Reads: the changed data rows (old contents), the new
+ *            rows and the parity rows; data rows outside `changed` are never loaded and may hold anything.  Every input word,
+ *            old or new, data or parity, is taken mod P.
+ *   Layout:  the three bases 16-byte aligned; the pitches and stripe strides multiples of 4 words; each pitch >= SIZE.  The call
+ *            accepts only layouts that fastecc_b200_rs_encode_batch's rule proves disjoint for the pairs (new, data), (new,
+ *            parity) and (data, parity): all N + M rows of all stripes pairwise disjoint and none of them meeting a new row.  New
+ *            rows may overlap each other (new_stripe_words = 0 gives every stripe the same new blocks).  Accepted: separate data,
+ *            parity and new spans, each stripe-major or block-major; one [B][N + M][pitch] stripe buffer with the new rows apart;
+ *            one [B][N + M + n_changed][pitch] buffer.  Anything else is EINVAL.
+ * PRECONDITION: as for fastecc_b200_rs_update, the stored parity is the encode of the stored data; fastecc_b200_rs_scrub checks it.
+ * Validated in full before anything is allocated or launched (EINVAL).  n_stripes == 0 or n_changed == 0 returns 0 and launches
+ * nothing (null buffers included).  Otherwise one kernel launch, plus the build of fastecc_b200_rs_update's table at the first
+ * use of an N; no workspace and no host-to-device copy (the list goes in the launch's parameters).  Asynchronous on the stream,
+ * which it does not synchronise; `changed` may be freed as soon as the call returns.
+ * Cost: it reads 2 n_changed + M rows and writes n_changed + M per stripe, with n_changed x M products per word.  Overwriting
+ * the changed rows and re-running fastecc_b200_rs_encode_batch reads N and writes M rows (plus the copy) with N x M products
+ * per word.  On an H100 (DESIGN 3n, 4 KiB blocks) this call is the faster one at every measured point except n_changed = N at
+ * N >= 48 with M >= 16 (48+16, 64+16, 64+64), where the re-encode is 1.05-1.19x faster; the crossing there lies between
+ * n_changed = N / 2 and N.  A caller that rewrites nearly whole stripes of those shapes should re-encode them. */
+int fastecc_b200_rs_update_batch(uint32_t* d_data, size_t data_pitch_words, size_t data_stripe_words, size_t N,
+                                 uint32_t* d_parity, size_t parity_pitch_words, size_t parity_stripe_words, size_t M,
+                                 const uint32_t* changed, size_t n_changed,
+                                 const uint32_t* d_new, size_t new_pitch_words, size_t new_stripe_words,
+                                 size_t n_stripes, size_t SIZE_words, void* stream);
+
 /* ---- one transform sharded over several GPUs (one process per GPU; BASELINE config 4) ---------------------------
  * Global block i = l*n_ranks + rank is local block l (data in, parity out).  An encode is: pass 0 on every rank,
  * all-to-all of whole blocks, pass 1, all-to-all, pass 2 -- the exchange is the caller's (fastecc_b200/sharded.py does it

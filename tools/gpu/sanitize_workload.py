@@ -62,6 +62,26 @@ for B, N, M, S, ld, lp in ((37, 12, 4, 7, [2, 11], [0]), (5, 64, 16, 1022, [0, 9
     out = fe.rs_reconstruct_batch_dev(data, par, ld, lp)
     for b in (0, B - 1):
         assert torch.equal(out[b], fe.rs_reconstruct_dev(data[b], par[b], ld, lp)), ("reconstruct batch", B, N, M, S, b)
+for B, N, M, S, ch in ((37, 12, 4, 7, [2, 11]), (5, 64, 16, 1022, [0, 9, 63]), (9, 18, 9, 33, list(range(18))),
+                      (6, 64, 1, 5, list(range(0, 64, 2)))):   # the batch update: M < 8 and M >= 8, SIZE % 4 != 0, row slices
+    data = torch.randint(-(1 << 31), 1 << 31, (B, N, (S + 3) // 4 * 4), dtype=torch.int32, device="cuda")[..., :S]
+    par = fe.rs_encode_batch_dev(data, M=M)
+    new = torch.randint(-(1 << 31), 1 << 31, (B, len(ch), (S + 3) // 4 * 4), dtype=torch.int32, device="cuda")[..., :S]
+    pad = lambda x: torch.empty((x.shape[0], (S + 3) // 4 * 4), dtype=torch.int32, device="cuda")[:, :S].copy_(x)
+    one = [(pad(data[b]), pad(par[b])) for b in (0, B - 1)]
+    fe.rs_update_batch_dev(data, par, ch, new)
+    for (d, p), b in zip(one, (0, B - 1)):
+        fe.rs_update_dev(d, p, ch, new[b])
+        assert torch.equal(par[b], p) and torch.equal(data[b], d), ("update batch", B, N, M, S, b)
+for B, N, M, S, ch in ((7, 12, 4, 7, [0, 5, 11]), (4, 32, 8, 130, [3])):   # one [B][N + M + k][pitch] buffer, updated in place
+    k, pitch = len(ch), (S + 3) // 4 * 4
+    buf = torch.randint(-(1 << 31), 1 << 31, (B, N + M + k, pitch), dtype=torch.int32, device="cuda")
+    fe.rs_encode_batch_dev(buf[:, :N, :S], buf[:, N:N + M, :S])
+    want = buf.clone()
+    want[:, ch, :S] = buf[:, N + M:, :S]
+    fe.rs_encode_batch_dev(want[:, :N, :S], want[:, N:N + M, :S])
+    fe.rs_update_batch_dev(buf[:, :N, :S], buf[:, N:N + M, :S], ch, buf[:, N + M:, :S])
+    assert torch.equal(buf[:, N:N + M, :S], want[:, N:N + M, :S]), ("update batch, one buffer", B, N, M, S)
 raw = torch.randint(0, 256, (64, 4096), dtype=torch.uint8, device="cuda")
 w = fe.bytes_to_gfp_dev(raw)
 assert bool((fe.gfp_to_bytes_dev(w, 1024) == raw).all())

@@ -6,7 +6,8 @@ Then recoding, decoding, the asymmetric encode, the encode of 3 * 2^k / 9 * 2^k 
 their encode into fewer parity blocks (`encode_asym_mixed`, DESIGN 3f; `--asym-mixed`: only these).  `--repair`: only the repair
 of a stored stripe against the 2N-row decoder (DESIGN 3g); `--update`, `--scrub`, `--scrub-degraded`, `--reconstruct`: only the update (3h),
 the scrub (3i), the degraded scrub (3j) or the degraded read (3k) lines; `--batch`: only the batch encode of small stripes (3l);
-`--reconstruct-batch`: only the degraded read of a batch of small stripes (3m).
+`--reconstruct-batch`: only the degraded read of a batch of small stripes (3m); `--update-batch`: only the update of a batch of
+small stripes in place (3n).
 Prints one JSON line per point."""
 import json
 import os
@@ -670,6 +671,61 @@ def reconstruct_batch_sweep():
         torch.cuda.empty_cache()
 
 
+def update_batch_sweep():
+    """Update of a batch of small stripes in place with one changed list (fastecc_b200_rs_update_batch, DESIGN 3n) at the shapes
+    of --batch, 4 KiB blocks, B stripes of about 1 GiB of data in all, data, parity and new rows in separate stripe-major buffers;
+    k changed blocks in {1, 2, N/4, N/2, N}.  The call: CUDA events around `reps` back-to-back calls (repeats write the same
+    words, so each does the same work), alternated twice with two other paths, the lower figures: (a) the new rows written into
+    the data with torch, then rs_encode_batch_dev of the stripes; (b) rs_update_dev stripe by stripe over the first `few`
+    stripes, events around the loop, scaled to B.  Floors: memory, (3 k + 2 M) * B * 4096 bytes at the data sheet's 3.35 TB/s
+    (k old rows read and written, k new rows read, M parity rows read and written); products, k * M * B * 1024 at the 1.7e12
+    products/s of update_parity_kernel (DESIGN 3h); the larger one binds.  "ok": the parity of three sampled stripes equals
+    rs_encode_asym_mixed_dev of their updated data.  Each line names the card and its power limit, read in the same run."""
+    from bench import gpu_identity
+    fe.init(0)
+    card = gpu_identity(torch.cuda.current_device())
+    S, few, reps = 1024, 300, 10
+    rng = np.random.default_rng(13)
+    for N, M in ((4, 2), (6, 3), (8, 4), (9, 3), (12, 4), (16, 4), (18, 3), (32, 8), (48, 16), (64, 16), (64, 64)):
+        B = (1 << 30) // (N * S * 4)
+        data = (torch.arange(B * N * S, device="cuda", dtype=torch.int64) * 2654435761 % P).to(torch.int32).view(B, N, S)
+        parity = torch.empty((B, M, S), dtype=torch.int32, device="cuda")
+        fe.rs_encode_batch_dev(data, parity)
+        for k in sorted({1, 2, max(N // 4, 1), max(N // 2, 1), N}):
+            changed = sorted(rng.choice(N, size=k, replace=False).tolist())
+            new = (torch.arange(B * k * S, device="cuda", dtype=torch.int64) * 40503 % P).to(torch.int32).view(B, k, S)
+            call = lambda: fe.rs_update_batch_dev(data, parity, changed, new)
+            call()
+            torch.cuda.synchronize()
+            ok = all(torch.equal(parity[b], _encode_one(data[b], M)) and torch.equal(data[b, changed], new[b]) for b in (0, B // 2, B - 1))
+
+            def overwrite_and_encode():
+                data[:, changed] = new
+                fe.rs_encode_batch_dev(data, parity)
+
+            def per_stripe():
+                for b in range(few):
+                    fe.rs_update_dev(data[b], parity[b], changed, new[b])
+            runs, runs_a, runs_b = [], [], []
+            for _ in range(2):
+                runs.append(timed(call, reps))
+                runs_a.append(timed(overwrite_and_encode, reps))
+                runs_b.append(timed(per_stripe, 2) * B / few)
+            ms, ms_a, ms_b = min(runs), min(runs_a), min(runs_b)
+            mem_ms = (3 * k + 2 * M) * B * S * 4 / 3.35e12 * 1e3
+            prod_ms = k * M * B * S / 1.7e12 * 1e3
+            print(json.dumps({"op": "update_batch", "N": N, "M": M, "B": B, "k": k, "block_bytes": 4 * S, "ok": ok, "call_ms": round(ms, 4),
+                              "call_ms_runs": [round(v, 4) for v in runs], "memory_floor_ms": round(mem_ms, 4), "product_floor_ms_at_1.7e12": round(prod_ms, 4),
+                              "binds": "memory" if mem_ms >= prod_ms else "products", "memory_floor_frac": round(mem_ms / ms, 3),
+                              "fraction_of_binding_floor": round(max(mem_ms, prod_ms) / ms, 3),
+                              "overwrite_encode_ms": round(ms_a, 4), "vs_overwrite_encode": round(ms_a / ms, 3),
+                              "per_stripe_ms_scaled_to_B": round(ms_b, 2), "per_stripe_stripes_timed": few, "speedup_vs_per_stripe": round(ms_b / ms, 1),
+                              "gpu": card["name"], "power_limit_w": card["power_limit_w"]}), flush=True)
+            del new
+        del data, parity
+        torch.cuda.empty_cache()
+
+
 def _encode_one(x, M):
     buf = x.clone()
     fe.rs_encode_asym_mixed_dev(buf, M)
@@ -677,6 +733,9 @@ def _encode_one(x, M):
 
 
 if __name__ == "__main__":
+    if "--update-batch" in sys.argv:                          # only the batch update lines
+        update_batch_sweep()
+        sys.exit(0)
     if "--reconstruct-batch" in sys.argv:                     # only the batched degraded read lines
         reconstruct_batch_sweep()
         sys.exit(0)
